@@ -1,4 +1,4 @@
-/* libmadstereo — C ABI of the B200-native real-time self-adaptive stereo engine.
+/* libmadstereo — C ABI of the H100-native real-time self-adaptive stereo engine.
  *
  * Drop-in boundary for ONE hot path of CVLAB-Unibo/Real-time-self-adaptive-deep-stereo: the per-frame
  * MADNet/DispNet forward + (MAD | FULL) backward + momentum update.  Every entry point names the reference
@@ -61,18 +61,8 @@ int ms_conv2d_fwd(const float* x, int n, int h, int w, int cin, int x_cs, const 
 int ms_conv2d_dgrad(const float* dy, int n, int oh, int ow, int cout, int dy_cs, const float* weights,
                     float* dx, int h, int w, int cin, int dx_cs, int kh, int kw, int stride, int dilation,
                     float* scratch, void* stream);
-/* tcgen05 (5th-gen tensor core, 3xTF32 split => fp32-grade accuracy) variants of the two ops above for
- * stride-1 convolutions; the engine uses them automatically for eligible layers (MS_CONV_TC=0 disables).
- * scratch: ms_conv2d_tc_scratch() floats.  Returns -3 if the shape is not eligible. */
-int ms_conv2d_fwd_tc(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights /*HWIO*/,
-                     const float* bias, float* y, int cout, int y_cs, int kh, int kw, int dilation, float alpha,
-                     float* scratch, size_t scratch_floats, void* stream);
-int ms_conv2d_dgrad_tc(const float* dy, int n, int h, int w, int cout, int dy_cs, const float* weights /*HWIO*/,
-                       float* dx, int cin, int dx_cs, int kh, int kw, int dilation, float* scratch,
-                       size_t scratch_floats, void* stream);
-size_t ms_conv2d_tc_scratch(int kh, int kw, int cin, int cout);
-/* Split-16-bit tcgen05 path (csrc/conv_bf.cu; the engine's default for every eligible layer, MS_CONV_IMPL=tf32 selects
- * the 3xTF32 kernels above): operands as two 16-bit planes (x ~= hi + lo), three kind::f16 MMAs per K step at the
+/* Split-16-bit wgmma path (csrc/conv_bf.cu; the engine's default for every eligible layer, MS_CONV_IMPL=fp32 selects
+ * the CUDA-core kernels above): operands as two 16-bit planes (x ~= hi + lo), three 16-bit MMAs per K step at the
  * bf16/fp16 tensor rate.  Forward operands are fp16 planes of x * act_scale and of w (22 mantissa bits, ~2^-22 relative
  * product error; the power-of-two scale is undone exactly in the epilogue); gradient operands are bf16 planes (16 bits, fp32 exponent
  * range).  GEMM transposed so that M = output channels and N = up to 256 pixels, halo patches by TMA (64-channel K
@@ -87,12 +77,12 @@ int ms_conv2d_dgrad_bf(const float* dy, int n, int oh, int ow, int cout, int dy_
                        float* dx, int h, int w, int cin, int dx_cs, int kh, int kw, int stride, int dilation,
                        void* scratch, size_t scratch_bytes, void* stream);
 size_t ms_conv2d_bf_scratch(int n, int h, int w, int kh, int kw, int cin, int cout);
-/* tcgen05 weight + bias gradient on the same planes (csrc/wgrad_bf.cu; the engine's default for eligible layers):
+/* wgmma weight + bias gradient on the same planes (csrc/wgrad_bf.cu; the engine's default for eligible layers):
  * replaces the filter / bias gradient sub-graphs of tf.nn.conv2d / atrous_conv2d / bias_add (reference
  * Nets/sharedLayers.py:58-59,72-73 under the train ops of Stereo_Online_Adaptation.py:118,128).  x and dy planes feed
- * the UMMA as MN-major operands straight from NHWC; stride 1 or 2, any dilation.  Same outputs as ms_conv2d_wgrad.
- * Both plane sets are bf16 (tcgen05 kind::f16 rejects an f16 x bf16 operand pair: probed, illegal instruction; the engine
- * therefore re-splits the forward activation into bf16 scratch planes for this kernel).
+ * the wgmma as MN-major operands straight from NHWC; stride 1 or 2, any dilation.  Same outputs as ms_conv2d_wgrad.
+ * Both plane sets are bf16 (a wgmma takes one 16-bit element type for both operands; the engine therefore re-splits the
+ * forward activation into bf16 scratch planes for this kernel).
  * scratch: ms_conv2d_wgrad_bf_scratch() BYTES, 256-byte aligned.  -3 = not eligible. */
 int ms_conv2d_wgrad_bf(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int oh, int ow, int cout,
                        int dy_cs, float* dw /*HWIO*/, float* db, int kh, int kw, int stride, int dilation,
@@ -118,11 +108,6 @@ int ms_conv2d_wgrad_bf_planes(const void* xhi, const void* xlo, int x_pcs, int n
                               const void* dhi, const void* dlo, int d_pcs, int oh, int ow, int cout, float* dw, float* db,
                               int kh, int kw, int stride, int dilation, float* workspace, size_t workspace_floats, void* stream);
 size_t ms_conv2d_wgrad_bf_workspace(int kh, int kw, int cin, int cout);
-/* tcgen05 weight gradient of a stride-1 conv (same outputs as ms_conv2d_wgrad); workspace from ..._workspace(). */
-int ms_conv2d_wgrad_tc(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int cout, int dy_cs,
-                       float* dw /*HWIO*/, float* db, int kh, int kw, int dilation, float* workspace,
-                       size_t workspace_floats, void* stream);
-size_t ms_conv2d_wgrad_tc_workspace(int kh, int kw, int cin, int cout, int n, int h, int w);
 size_t ms_conv2d_wgrad_workspace(int kh, int kw, int cin, int cout, size_t out_pixels);
 int ms_conv2d_wgrad(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int oh, int ow,
                     int cout, int dy_cs, float* dw /*HWIO*/, float* db, int kh, int kw, int stride,
@@ -142,7 +127,7 @@ size_t ms_conv2d_stem_wgrad_workspace(int n, int h, int w);
 int ms_conv2d_stem_wgrad(const float* x4, int n, int h, int w, const float* dy, int dy_cs, float* dw, float* db, float* workspace,
                          size_t workspace_floats, void* stream);
 
-/* The same layer and its two gradients on the split-16-bit tcgen05 path (csrc/conv_bf.cu, csrc/wgrad_bf.cu): forward as a
+/* The same layer and its two gradients on the split-16-bit wgmma path (csrc/conv_bf.cu, csrc/wgrad_bf.cu): forward as a
  * fractionally strided gather in four output-parity launches (fp16 planes of x*act_scale), input gradient as the
  * stride-`stride` conv of dy with the filter read as HWIO [kh,kw,cout,cin], weight gradient as that conv's wgrad with the
  * big map in the activation role (both bf16 planes).  dy [n,h*stride,w*stride,cout]; dw [kh,kw,cout,cin]; db [cout] or NULL.
@@ -259,18 +244,6 @@ float ms_engine_profile_event_overhead_ms(void* e);
 int ms_engine_profile_read(void* e, double* ms7, double* macs7, double* bytes7, long long* calls7);
 /* Kernels launched by this library in this process so far. */
 long long ms_launch_count(void);
-/* Diagnostic (no reference counterpart): per-role clock64 counters of the tcgen05 conv kernel, filled only when the
- * environment selects its profiling build (MS_TC_DEBUG=8, scripts/tc_prof.py). out32: 32 counters; reset != 0 clears. */
-int ms_debug_tc_prof(unsigned long long* out32, int reset);
-/* Diagnosis: cycles per tcgen05.mma.kind::f16 (M = 128, K = 16, bf16) issued back to back by one thread per CTA on zeroed
- * shared memory, for K-major / MN-major operand layouts, MMA N, number of accumulators visited round-robin, and the
- * issue scheme (uni = 0: loop on lane 0 only; 1: warp-uniform loop, elected lane issues).  out_dev:
- * 2 * ctas int64 (issue-loop cycles, cycles until the last MMA retired).  scripts/mma_probe.py prints the table. */
-int ms_debug_mma_probe(int a_mn, int b_mn, int n, int n_acc, int rot, int iters, int uni, int ctas, long long* out_dev, void* stream);
-
-/* MS_BF_PROF=1: clock64 stamps of the last conv_bf launch, 8 per CTA (entry, setup done, first data, MMAs issued,
- * accumulator seen, epilogue done, exit, MMA-thread wait cycles); returns the number of CTAs copied */
-int ms_debug_bf_prof(unsigned long long* out, int max_ctas);
 int ms_engine_num_tensors(void* e);
 int ms_engine_tensor_name(void* e, int i, char* name, int cap);
 /* dims: n,h,w,c,cs */

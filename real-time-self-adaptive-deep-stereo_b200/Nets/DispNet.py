@@ -1,4 +1,4 @@
-"""DispNet-C on the B200 engine — host-side mirror of the reference class (Nets/DispNet.py:9-152).
+"""DispNet-C on the H100 engine — host-side mirror of the reference class (Nets/DispNet.py:9-152).
 
 Same construction API / argument validation (DispNet.py:23-37) / layer names (`conv1a`, `conv3/1`, `up5/deconv`, ...)
 and `get_disparities()` ordering (5 side predictions, `prediction`, `rescaled_prediction`).  The graph itself

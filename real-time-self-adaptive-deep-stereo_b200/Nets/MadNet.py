@@ -1,4 +1,4 @@
-"""MADNet on the B200 engine — host-side mirror of the reference class (Nets/MadNet.py:8-436).
+"""MADNet on the H100 engine — host-side mirror of the reference class (Nets/MadNet.py:8-436).
 
 Construction API, argument validation, layer names and `get_disparities()` ordering follow the reference;
 the graph itself (pyramid :173-249, warp/correlation/estimator loop :251-351, context net :122-171, outputs

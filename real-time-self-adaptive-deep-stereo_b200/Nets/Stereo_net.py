@@ -147,7 +147,7 @@ class StereoNet(object):
         if args['train_portion'] not in ('BEGIN', 'END'):
             raise Exception('Invalid portion options {}'.format(args['train_portion']))
         if args['split_layers'] != [None]:
-            raise Exception('split_layers other than [None] is not supported by the B200 engine '
+            raise Exception('split_layers other than [None] is not supported by the H100 engine '
                             '(the adaptation drivers always pass [None], Stereo_Online_Adaptation.py:57)')
         self._split_layers_list = args['split_layers']
         self._train_beginning = args['train_portion'] == 'BEGIN'

@@ -1,4 +1,4 @@
-"""Continual online adaptation with proxy supervision -- the reference's TPAMI driver on the B200 engine.
+"""Continual online adaptation with proxy supervision -- the reference's TPAMI driver on the H100 engine.
 
 Mirrors Stereo_Continual_Adaptation.py of the reference: the same flags (:309-330, incl. --dilation / --decay / --uf /
 --saveWeights / --eval), list files `left;right;gt;proxy`, the loss `get_proxy_loss('mean_l1')` (masked L1 to proxy

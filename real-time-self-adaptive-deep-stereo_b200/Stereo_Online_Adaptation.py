@@ -1,4 +1,4 @@
-"""Online adaptation of a deep stereo network -- the reference driver's command line on the B200 engine.
+"""Online adaptation of a deep stereo network -- the reference driver's command line on the H100 engine.
 
 Mirrors Stereo_Online_Adaptation.py of the reference: the same flags (:290-307), the same output folder layout
 (`config.json`, `params.sh`, `stats.csv`, `series.csv`, `disparities/disparity_<step>.png`, :262-288, :309-319) and the

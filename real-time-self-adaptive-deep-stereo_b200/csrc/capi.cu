@@ -40,9 +40,6 @@ int ms_corr_fwd(const float* left, int left_cs, const float* right, int right_cs
     return corr_fwd(p, S(stream));
 }
 
-int ms_debug_mma_probe(int a_mn, int b_mn, int n, int n_acc, int rot, int iters, int uni, int ctas, long long* out_dev, void* stream) {
-    return mma_probe(a_mn, b_mn, n, n_acc, rot, iters, uni, ctas, out_dev, S(stream));
-}
 int ms_corr_fwd_wide(const float* left, int left_cs, const float* right, int right_cs, float* out, int out_cs, int B, int h,
                      int w, int C, int max_disp, float act_scale, void* stream) {
     CorrFwd p{};
@@ -98,36 +95,6 @@ int ms_conv2d_dgrad(const float* dy, int n, int oh, int ow, int cout, int dy_cs,
     return conv_gemm(p, S(stream));
 }
 
-int ms_conv2d_fwd_tc(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights, const float* bias,
-                     float* y, int cout, int y_cs, int kh, int kw, int dilation, float alpha, float* scratch,
-                     size_t scratch_floats, void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, kh, 1, dilation, oh, pt);
-    same_pad_c(w, kw, 1, dilation, ow, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    p.y = view(y, n, oh, ow, cout, y_cs);
-    p.wmat = weights; p.bias = bias; p.kh = kh; p.kw = kw;
-    p.mul = 1; p.off_y = -pt; p.off_x = -pl; p.step = dilation; p.div = 1;
-    p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
-    if (!conv_tc_supported(p)) { set_error("ms_conv2d_fwd_tc: shape not supported by the tcgen05 path"); return -3; }
-    return conv_tc_oneshot(p, 0, scratch, scratch_floats, S(stream));
-}
-int ms_conv2d_dgrad_tc(const float* dy, int n, int h, int w, int cout, int dy_cs, const float* weights, float* dx,
-                       int cin, int dx_cs, int kh, int kw, int dilation, float* scratch, size_t scratch_floats,
-                       void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, kh, 1, dilation, oh, pt);
-    same_pad_c(w, kw, 1, dilation, ow, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(dy), n, h, w, cout, dy_cs);
-    p.y = view(dx, n, h, w, cin, dx_cs);
-    p.wmat = weights; p.bias = nullptr; p.kh = kh; p.kw = kw;
-    p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -dilation; p.div = 1;
-    p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
-    if (!conv_tc_supported(p)) { set_error("ms_conv2d_dgrad_tc: shape not supported by the tcgen05 path"); return -3; }
-    return conv_tc_oneshot(p, 1, scratch, scratch_floats, S(stream));
-}
 int ms_conv2d_fwd_bf(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights, const float* bias,
                      float* y, int cout, int y_cs, int kh, int kw, int stride, int dilation, float alpha, float act_scale,
                      void* scratch, size_t scratch_bytes, void* stream) {
@@ -140,7 +107,7 @@ int ms_conv2d_fwd_bf(const float* x, int n, int h, int w, int cin, int x_cs, con
     p.wmat = weights; p.bias = bias; p.kh = kh; p.kw = kw;
     p.mul = stride; p.off_y = -pt; p.off_x = -pl; p.step = dilation; p.div = 1;
     p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
-    if (!conv_bf_supported(p)) { set_error("ms_conv2d_fwd_bf: shape not supported by the split-bf16 tcgen05 path"); return -3; }
+    if (!conv_bf_supported(p)) { set_error("ms_conv2d_fwd_bf: shape not supported by the split-16-bit tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 0, 1, act_scale, scratch, scratch_bytes, S(stream));      // forward: fp16 planes of x * act_scale
 }
 int ms_conv2d_dgrad_bf(const float* dy, int n, int oh, int ow, int cout, int dy_cs, const float* weights, float* dx,
@@ -156,7 +123,7 @@ int ms_conv2d_dgrad_bf(const float* dy, int n, int oh, int ow, int cout, int dy_
     p.wmat = weights; p.bias = nullptr; p.kh = kh; p.kw = kw;
     p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -dilation; p.div = stride;
     p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
-    if (!conv_bf_supported(p)) { set_error("ms_conv2d_dgrad_bf: shape not supported by the split-bf16 tcgen05 path"); return -3; }
+    if (!conv_bf_supported(p)) { set_error("ms_conv2d_dgrad_bf: shape not supported by the split-16-bit tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 1, 0, 1.f, scratch, scratch_bytes, S(stream));      // gradients: bf16 planes
 }
 size_t ms_conv2d_bf_scratch(int n, int h, int w, int kh, int kw, int cin, int cout) {
@@ -178,7 +145,7 @@ int ms_conv2d_wgrad_bf(const float* x, int n, int h, int w, int cin, int x_cs, c
     q.dy = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);
     q.dw = dw; q.db = db; q.kh = kh; q.kw = kw; q.stride = stride; q.dil = dilation; q.pad_t = pt; q.pad_l = pl;
     q.accumulate = 0;
-    if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_wgrad_bf: shape not supported by the split-bf16 tcgen05 path"); return -3; }
+    if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_wgrad_bf: shape not supported by the split-16-bit tensor-core path"); return -3; }
     return wgrad_bf_oneshot(q, scratch, scratch_bytes, S(stream));
 }
 size_t ms_conv2d_wgrad_bf_scratch(int n, int h, int w, int oh, int ow, int kh, int kw, int cin, int cout) {
@@ -221,7 +188,7 @@ int ms_conv2d_stem_wgrad(const float* x4, int n, int h, int w, const float* dy, 
     return conv_stem_wgrad(q, S(stream));
 }
 
-// ---- conv2d_transpose (Nets/sharedLayers.py:80-92) and its two gradients on the split-16-bit tcgen05 path.
+// ---- conv2d_transpose (Nets/sharedLayers.py:80-92) and its two gradients on the split-16-bit tensor-core path.
 //      weights [kh,kw,cout,cin] (TF layout); x [n,h,w,cin]; y / dy [n,h*stride,w*stride,cout]
 static void transpose_geom(int h, int w, int kh, int kw, int stride, int& oh, int& ow, int& pt, int& pl) {
     oh = h * stride; ow = w * stride;
@@ -240,7 +207,7 @@ int ms_conv2d_transpose_fwd_bf(const float* x, int n, int h, int w, int cin, int
     p.wmat = weights; p.bias = bias; p.kh = kh; p.kw = kw;
     p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = stride;
     p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
-    if (!conv_bf_supported(p)) { set_error("ms_conv2d_transpose_fwd_bf: shape not supported by the tcgen05 path"); return -3; }
+    if (!conv_bf_supported(p)) { set_error("ms_conv2d_transpose_fwd_bf: shape not supported by the tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 1, 1, act_scale, scratch, scratch_bytes, S(stream));     // [tap][M = cout][K = cin], fp16 planes
 }
 int ms_conv2d_transpose_dgrad_bf(const float* dy, int n, int h, int w, int cout, int dy_cs, const float* weights, float* dx,
@@ -254,7 +221,7 @@ int ms_conv2d_transpose_dgrad_bf(const float* dy, int n, int h, int w, int cout,
     p.wmat = weights; p.bias = nullptr; p.kh = kh; p.kw = kw;
     p.mul = stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1;      // = the strided conv of dy with HWIO [.,.,cout,cin]
     p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
-    if (!conv_bf_supported(p)) { set_error("ms_conv2d_transpose_dgrad_bf: shape not supported by the tcgen05 path"); return -3; }
+    if (!conv_bf_supported(p)) { set_error("ms_conv2d_transpose_dgrad_bf: shape not supported by the tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 0, 0, 1.f, scratch, scratch_bytes, S(stream));           // [tap][K = cout][M = cin], bf16 planes
 }
 size_t ms_conv2d_transpose_bf_scratch(int n, int h, int w, int kh, int kw, int cin, int cout, int stride) {
@@ -283,7 +250,7 @@ int ms_conv2d_transpose_wgrad_bf(const float* x, int n, int h, int w, int cin, i
                                  void* stream) {
     ConvWgrad q = transpose_wgrad_geom(x, n, h, w, cin, x_cs, dy, cout, dy_cs, kh, kw, stride);
     q.dw = dw; q.db = nullptr;                                        // dw [kh,kw,cout,cin]
-    if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_transpose_wgrad_bf: shape not supported by the tcgen05 path"); return -3; }
+    if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_transpose_wgrad_bf: shape not supported by the tensor-core path"); return -3; }
     if (wgrad_bf_oneshot(q, scratch, scratch_bytes, S(stream))) return -1;
     if (!db) return 0;
     // bias gradient = per-channel sum of dy; the partial-sum region of the scratch is free again after the reduction
@@ -343,10 +310,6 @@ int ms_conv2d_wgrad_bf_planes(const void* xhi, const void* xlo, int x_pcs, int n
     return wgrad_bf(q, xp, dp, S(stream));
 }
 size_t ms_conv2d_wgrad_bf_workspace(int kh, int kw, int cin, int cout) { return wgrad_bf_workspace_floats(kh, kw, cin, cout); }
-size_t ms_conv2d_tc_scratch(int kh, int kw, int cin, int cout) {
-    size_t a = conv_tc_scratch_floats(kh * kw, cout, cin), b = conv_tc_scratch_floats(kh * kw, cin, cout);
-    return a > b ? a : b;
-}
 
 size_t ms_conv2d_wgrad_workspace(int kh, int kw, int cin, int cout, size_t out_pixels) {
     return conv_wgrad_workspace_floats(kh * kw, cin, cout, out_pixels);
@@ -365,24 +328,6 @@ int ms_conv2d_wgrad(const float* x, int n, int h, int w, int cin, int x_cs, cons
     q.dw = dw; q.db = db; q.kh = kh; q.kw = kw; q.stride = stride; q.dil = dilation; q.pad_t = pt; q.pad_l = pl;
     q.workspace = workspace; q.workspace_floats = workspace_floats; q.accumulate = 0;
     return conv_wgrad(q, S(stream));
-}
-
-int ms_conv2d_wgrad_tc(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int cout, int dy_cs,
-                       float* dw, float* db, int kh, int kw, int dilation, float* workspace, size_t workspace_floats,
-                       void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, kh, 1, dilation, oh, pt);
-    same_pad_c(w, kw, 1, dilation, ow, pl);
-    ConvWgrad q{};
-    q.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    q.dy = view(const_cast<float*>(dy), n, h, w, cout, dy_cs);
-    q.dw = dw; q.db = db; q.kh = kh; q.kw = kw; q.stride = 1; q.dil = dilation; q.pad_t = pt; q.pad_l = pl;
-    q.workspace = workspace; q.workspace_floats = workspace_floats; q.accumulate = 0;
-    if (!wgrad_tc_supported(q)) { set_error("ms_conv2d_wgrad_tc: shape not supported by the tcgen05 path"); return -3; }
-    return wgrad_tc(q, S(stream));
-}
-size_t ms_conv2d_wgrad_tc_workspace(int kh, int kw, int cin, int cout, int n, int h, int w) {
-    return wgrad_tc_workspace_floats(kh * kw, cin, cout, n, h, w);
 }
 
 int ms_conv2d_transpose_fwd(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights,
@@ -502,9 +447,6 @@ int ms_engine_bind(void* h, float* weights, float* grads, float* momentum, float
     if (e->layout(workspace) > need) { set_error("ms_engine_bind: layout exceeds the size reported by ms_engine_sizes"); return -2; }
     MS_CHECK_CUDA(cudaMemsetAsync(workspace, 0, need * sizeof(float), S(stream)));
     MS_CHECK_CUDA(cudaMemsetAsync(grads, 0, e->n_params * sizeof(float), S(stream)));
-    if (!e->prep_jobs.empty())
-        MS_CHECK_CUDA(cudaMemcpyAsync(e->prep_jobs_dev, e->prep_jobs.data(), e->prep_jobs.size() * sizeof(TcPrepJob),
-                                      cudaMemcpyHostToDevice, S(stream)));
     if (!e->bf_jobs.empty())
         MS_CHECK_CUDA(cudaMemcpyAsync(e->bf_jobs_dev, e->bf_jobs.data(), e->bf_jobs.size() * sizeof(BfPrepJob),
                                       cudaMemcpyHostToDevice, S(stream)));
@@ -606,8 +548,6 @@ int ms_engine_profile_layers(void* h, double* ms3n, long long* calls3n) {
 }
 float ms_engine_profile_event_overhead_ms(void* h) { return static_cast<Engine*>(h)->prof_event_overhead_ms; }
 long long ms_launch_count(void) { return ms::launch_count(); }
-int ms_debug_tc_prof(unsigned long long* out32, int reset) { return ms::conv_tc_read_prof(out32, reset); }
-int ms_debug_bf_prof(unsigned long long* out, int max_ctas) { return ms::conv_bf_read_prof(out, max_ctas); }
 int ms_engine_num_tensors(void* h) { return (int)static_cast<Engine*>(h)->tensors.size(); }
 int ms_engine_tensor_name(void* h, int i, char* name, int cap) {
     Engine* e = static_cast<Engine*>(h);

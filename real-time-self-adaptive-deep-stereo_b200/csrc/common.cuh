@@ -1,4 +1,4 @@
-// Shared declarations for libmadstereo (sm_100a only).
+// Shared declarations for libmadstereo (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,8 +47,8 @@ void add_launches(long long n);
 // launch_k(), which sets cudaLaunchAttributeProgrammaticStreamSerialization (MS_PDL=0 disables).  A kernel's CTAs may
 // then become resident while the previous kernel of the stream is still draining; nothing of the kernel body runs before
 // that kernel has completed and flushed (griddepcontrol.wait), so the data dependences of the stream order are intact --
-// what overlaps is launch latency and, in the tcgen05 kernels, barrier / TMEM set-up.  Inside the captured step graph the
-// attribute becomes a programmatic edge.  Measured on the conv -> conv edges alone: 551 -> 561 FPS.
+// what overlaps is launch latency and, in the tensor-core kernels, barrier set-up.  Inside the captured step graph the
+// attribute becomes a programmatic edge.
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -71,6 +71,10 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
     carveout_once(reinterpret_cast<const void*>(kernel));
     (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);      // errors surface in check_launch()
 }
+
+// streaming multiprocessors of the H100 SXM: grid sizing and split heuristics (a workspace sized from it must match the
+// grid it serves, so it is one constant rather than a device query)
+constexpr int NUM_SMS = 132;
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 static inline size_t cdivz(size_t a, size_t b) { return (a + b - 1) / b; }
@@ -96,6 +100,7 @@ struct ConvGemm {
     int ksplit;           // set by conv_gemm()
 };
 int conv_gemm(const ConvGemm& p, cudaStream_t st);
+size_t conv_gemm_part_floats();       // split-K scratch the engine provides to conv_gemm
 
 struct ConvWgrad {
     TView x;              // forward-conv input   [n, xh, xw, ci]
@@ -144,7 +149,6 @@ struct CorrFwd {
                                      // tensor-core kernel for wide windows (corr_mma.cu); 0: CUDA-core kernels only
 };
 int corr_fwd(const CorrFwd& p, cudaStream_t st);
-int mma_probe(int a_mn, int b_mn, int n, int n_acc, int rot, int iters, int uni, int ctas, long long* out_dev, cudaStream_t st);   // wgrad_bf.cu (diagnosis)
 bool corr_mma_supported(const CorrFwd& p);          // corr_mma.cu: wide window (>= 17 displacements), no warp, stride 1
 int corr_mma(const CorrFwd& p, cudaStream_t st);
 int corr_fwd4(const CorrFwd& p, cudaStream_t st);   // corr_tma.cu: 0 launched, 1 shape not handled, -1 error
@@ -207,30 +211,8 @@ int momentum_update(float* w, const float* g, float* m, size_t n, float lr, floa
 }  // namespace ms
 
 namespace ms {
-// tcgen05 path (conv_tc.cu)
-struct TcPrepJob {
-    const float* src; float* bh; float* bl;
-    int taps, N, K, BN, Kpad, transposed_src;
-};
-bool conv_tc_supported(const ConvGemm& g);
-void conv_tc_weight_dims(int N, int K, int& BN, int& Kpad);
-size_t conv_tc_scratch_floats(int taps, int N, int K);
-int conv_tc_init();
-int tc_prep_weights(const TcPrepJob* jobs_dev, int njobs, size_t max_total, cudaStream_t st);
-int conv_tc(const ConvGemm& g, const float* bw, cudaStream_t st, float* part);
-size_t conv_tc_part_floats();
-bool conv_tc_profitable(const ConvGemm& g);
-int conv_tc_oneshot(const ConvGemm& g, int wmat_is_nk, float* scratch, size_t scratch_floats, cudaStream_t st);
 int corr_init();
-bool wgrad_tc_supported(const ConvWgrad& q);
-size_t wgrad_tc_workspace_floats(int taps, int ci, int co, int n, int h, int w);
-int wgrad_tc_init();
-int wgrad_tc(const ConvWgrad& q, cudaStream_t st);
-int conv_tc_read_prof(unsigned long long* out32, int reset);
-}  // namespace ms
-
-namespace ms {
-// split-bf16 tcgen05 path (conv_bf.cu): every activation that feeds a convolution also lives as two bf16 planes
+// split-bf16 wgmma path (conv_bf.cu): every activation that feeds a convolution also lives as two bf16 planes
 // (hi = bf16(x), lo = bf16(x - hi)), NHWC with channel stride `cs` (bf16 elements, multiple of 8).
 struct ActPlanes { void* hi; void* lo; int cs; int fmt; float scale; };   // fmt 0 = bf16 (gradients), 1 = fp16 of x * scale (forward activations; scale a power of two)
 struct BfPrepJob {
@@ -247,12 +229,11 @@ size_t conv_bf_weight_halfs(int taps, int M, int K);
 size_t conv_bf_part_floats();
 size_t conv_bf_ticket_words();
 int conv_bf_init();
-int conv_bf_read_prof(unsigned long long* out, int max_ctas);
 int bf_prep_weights(const BfPrepJob* jobs_dev, int njobs, size_t max_total, cudaStream_t st);
 int split_planes(const TView& x, const ActPlanes& pl, cudaStream_t st);
 int conv_bf(const ConvGemm& g, const ActPlanes& xp, const void* wtiles, const ActPlanes* yp, float* part,
             unsigned int* tickets, cudaStream_t st);
-// wgrad_bf.cu: weight + bias gradient on the same planes (MN-major UMMA operands, no transposes)
+// wgrad_bf.cu: weight + bias gradient on the same planes (MN-major wgmma operands, no transposes)
 bool wgrad_bf_supported(const ConvWgrad& q);
 size_t wgrad_bf_workspace_floats(int kh, int kw, int ci, int co);
 int wgrad_bf_init();

@@ -1,11 +1,11 @@
-// fp32 CUDA-core implicit-GEMM convolution family (sm_100a).
+// fp32 CUDA-core implicit-GEMM convolution family (sm_90a).
 //
 // Replaces, for the hot path, the cuDNN calls behind tf.nn.conv2d / atrous_conv2d / conv2d_transpose
 // (reference Nets/sharedLayers.py:54-92) and the conv gradients tf.gradients derives for them.
 // One "gather GEMM" kernel serves conv forward, conv dgrad and conv_transpose forward (see ConvGemm in
 // common.cuh); a second kernel computes weight gradients as a split-K GEMM over pixels with a
 // deterministic two-pass reduction.  This is the exact-fp32 path: it is used for every layer shape the
-// tcgen05 path (conv_tc.cu) does not cover (stride 2, cin=3, cout=1, transposed) and as its checker.
+// split-16-bit tensor-core path (conv_bf.cu) does not cover and as its checker.
 #include "common.cuh"
 #include <algorithm>
 #include <cstdlib>
@@ -246,6 +246,8 @@ __global__ void gemm_splitk_reduce_kernel(ConvGemm p, int M) {
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+size_t conv_gemm_part_floats() { return (size_t)8 << 20; }      // 32 MB split-K partial-sum scratch
+
 int conv_gemm(const ConvGemm& p_in, cudaStream_t st) {
     ConvGemm p = p_in;
     MS_REQUIRE(p.x.n == p.y.n, "conv_gemm: batch mismatch");
@@ -265,7 +267,7 @@ int conv_gemm(const ConvGemm& p_in, cudaStream_t st) {
     p.ksplit = 1;
     {
         const int ctas = grid.x * grid.y, total_k = p.kh * p.kw * cdiv(p.x.c, BK);
-        if (p.part && ctas <= 74 && total_k >= 8) {
+        if (p.part && ctas <= NUM_SMS / 2 && total_k >= 8) {
             int ks = std::min(total_k / 4, std::max(1, 296 / ctas));
             if (ks > 32) ks = 32;
             if (ks > 1 && (size_t)ks * M * p.y.c <= p.part_floats) { p.ksplit = ks; grid.z = ks; }
@@ -483,7 +485,7 @@ size_t conv_wgrad_workspace_floats(int taps, int ci, int co, size_t P) {
     int tiles = taps * cdiv(ci, 16 * tm) * cdiv(co, 16 * tn);
     size_t main_part = (size_t)wgrad_split(tiles, P) * taps * ci * co;
     if (conv_small_wgrad_shape(taps, ci, co)) main_part = std::max(main_part, conv_small_wgrad_workspace_floats(taps, ci, co, P));
-    if (co == 1) main_part = std::max(main_part, (size_t)2 * 148 * ((size_t)taps * ci + 1));      // conv_head_wgrad partials
+    if (co == 1) main_part = std::max(main_part, (size_t)2 * NUM_SMS * ((size_t)taps * ci + 1));      // conv_head_wgrad partials
     return main_part + (size_t)bias_blocks(P) * co + 64;
 }
 

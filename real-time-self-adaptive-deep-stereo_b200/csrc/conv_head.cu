@@ -3,7 +3,7 @@
 // Replaces the cuDNN calls behind the linear 3x3 -> 1 convolutions of the reference: estimator `disp-6`
 // (Nets/MadNet.py:113-118), `context-7` with the residual add (:160-168), DispNet `predict` / `prediction`
 // (Nets/DispNet.py:49-50,143-146), and their input gradients (1 -> cin).  Round 1 ran these through the generic fp32
-// gather GEMM (68 us per launch at 96x320x32); here a pixel's channel vector is one coalesced 128-bit load per lane.
+// gather GEMM; here a pixel's channel vector is one coalesced 128-bit load per lane.
 #include <algorithm>
 
 #include "common.cuh"
@@ -102,8 +102,8 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 // 1 = forward head (y.c == 1), 2 = head dgrad (x.c == 1), 0 = not a head
 // single-channel gather (1 -> 1 channel, any generic gather geometry): DispNet's `up_predict` 4x4 stride-2 conv_transpose of
-// a disparity map (Nets/DispNet.py:51-53).  One thread per output pixel; the generic fp32 gather GEMM spent 166 us on the
-// 192x640 instance of this 2 MFLOP operation.
+// a disparity map (Nets/DispNet.py:51-53).  One thread per output pixel; the generic fp32 gather GEMM is far too slow for
+// this 2 MFLOP operation.
 __global__ void __launch_bounds__(256) conv_one_channel_kernel(ConvGemm g, size_t npix) {
     pdl_prologue();
     const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -143,7 +143,7 @@ int conv_one_channel(const ConvGemm& g, cudaStream_t st) {
 // weight (+ bias) gradient of a conv with ONE output channel: dw[tap][c] = sum_p x[p * stride - pad + tap * dil][c] * dy[p].
 // (DispNet `prediction` 32 -> 1 at 192 x 640, `predict` heads, the 1 -> 1 `up_predict` transposed convs with the big map
 // in the x role; MADNet `disp-6` / `context-7`.)  288 ... 16 k outputs reduced over up to 123 k pixels: the generic fp32
-// wgrad GEMM pads co = 1 to a 16-wide tile (156 us for `prediction`); here G lanes share a pixel (4 channels each), every
+// wgrad GEMM pads co = 1 to a 16-wide tile; here G lanes share a pixel (4 channels each), every
 // thread keeps its K x K x 4 partial sums in registers over a grid-stride pixel loop, and the CTA folds them in a fixed
 // order (deterministic) into one partial vector.
 template <int K>
@@ -229,7 +229,7 @@ static int head_wgrad_grid(const ConvWgrad& q, int& gshift) {
     gshift = 0;
     while ((1 << gshift) < c4) ++gshift;
     const size_t pp = 256 >> gshift;
-    return (int)std::min<size_t>(cdivz(q.dy.pixels(), pp), 2 * 148);
+    return (int)std::min<size_t>(cdivz(q.dy.pixels(), pp), 2 * NUM_SMS);
 }
 bool conv_head_wgrad_supported(const ConvWgrad& q) {
     return q.dy.c == 1 && q.kh == q.kw && (q.kh == 3 || q.kh == 4) && q.x.c >= 1 && q.x.c <= 1024 && q.x.n == q.dy.n;
@@ -289,7 +289,7 @@ int conv_head(const ConvGemm& g, cudaStream_t st) {
         return check_launch("conv_head_fwd");
     }
     const size_t total = npix * (g.y.c >> 2);
-    const unsigned grid = (unsigned)std::min<size_t>(cdivz(total, 256), 148 * 8);
+    const unsigned grid = (unsigned)std::min<size_t>(cdivz(total, 256), NUM_SMS * 8);
     launch_k(conv_head_dgrad_kernel, dim3(grid), dim3(256), smem, st, g, npix);
     return check_launch("conv_head_dgrad");
 }

@@ -3,11 +3,11 @@
 // sharedLayers.conv2d (Nets/sharedLayers.py:54-63), and the filter gradients tf.gradients derives for them in the
 // module-2 train op (Stereo_Online_Adaptation.py:118).
 //
-// The launch list (profiles/r1_launches_final_summary.txt) had the gather GEMM at 105 us for conv1 forward (0.2 GFLOP,
-// 27 MB: it should be a ~10 us HBM-bound kernel) and 319 + 271 us for the conv1 / conv2 weight gradients (432 / 2304
-// outputs reduced over 245 760 pixels: a 16 x 16 output tile leaves the GEMM kernel with 9 CTAs per K split).
+// On these layers the generic gather GEMM is far from the HBM bound for conv1 forward (0.2 GFLOP, 27 MB) and for the
+// conv1 / conv2 weight gradients (432 / 2304 outputs reduced over 245 760 pixels: a 16 x 16 output tile leaves the GEMM
+// kernel with 9 CTAs per K split).
 //   forward  : one thread computes two adjacent output pixels x all output channels; the weights sit in shared memory
-//              and are read as broadcast float4.  105 -> 30 us for conv1.  (16 -> 16 | 32 instantiations exist but are
+//              and are read as broadcast float4.  (16 -> 16 | 32 instantiations exist but are
 //              opt-in: without a staged input patch they are slower than the gather GEMM, see conv_small_fwd_supported.)
 //   wgrad    : a thread owns one input channel ("role") and keeps all 9 taps x 16 output channels = 144 partial sums
 //              in registers while it walks its share of the pixels (9 input loads + 16 dY loads per 144 FMAs, next
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(CS_NT) conv_small_fwd_kernel(ConvGemm p, int p
 // the 10 x 34 input patch is loaded with coalesced 128-bit loads into shared memory with a 20-float pixel pitch (a
 // quarter-warp's 128-bit reads at one-pixel lane stride then hit 32 distinct banks); a thread computes pixels (r, c) and
 // (r, c + 16) so that lanes stay one pixel apart.  Default (MS_CONV_SMALL16=2; 0 = gather GEMM, 1 = untiled direct
-// kernels): validated with the ops + MADNet GPU suites, conv_fwd 1.600 -> 1.575 ms per frame (profiles/r1_last_visit.log).
+// kernels): validated with the ops + MADNet GPU suites.
 // ---------------------------------------------------------------------------------------------
 constexpr int T16_TH = 8, T16_TW = 32, T16_PH = T16_TH + 2, T16_PW = T16_TW + 2, T16_PS = 20, T16_NT = 128;
 
@@ -216,9 +216,9 @@ static bool conv_c16_tiled_supported(const ConvGemm& p) {
 bool conv_small_fwd_supported(const ConvGemm& p) {
     if (p.kh != 3 || p.kw != 3 || p.div != 1 || p.mul < 1 || p.x.n != p.y.n || p.alpha > 1.f || p.alpha < 0.f) return false;
     if (p.x.c == 3 && p.y.c == 16) return true;
-    // The untiled 16-channel instantiations are opt-in (MS_CONV_SMALL16=1): measured 86 us (16->16) and 36 us (16->32
-    // stride 2) against 71 / 32 us for the gather GEMM -- one thread reading its pixels' 64-byte channel rows straight
-    // from global memory is LSU-bound (32 cache lines per load instruction).  The default (=2) is the shared-memory
+    // The untiled 16-channel instantiations are opt-in (MS_CONV_SMALL16=1): slower than the gather GEMM -- one thread
+    // reading its pixels' 64-byte channel rows straight from global memory is LSU-bound (32 cache lines per load
+    // instruction).  The default (=2) is the shared-memory
     // tiled 16->16 stride-1 kernel above.
     if (small16_mode() == 2 && conv_c16_tiled_supported(p)) return true;
     if (small16_mode() == 1 && p.x.c == 16 && (p.y.c == 16 || p.y.c == 32)) return (p.x.cs & 3) == 0 && al16s(p.x.p);
@@ -354,7 +354,7 @@ __global__ void __launch_bounds__(SW_NT, 1) conv_small_wgrad_kernel(ConvWgrad p,
 
 bool conv_small_wgrad_shape(int taps, int ci, int co) { return taps == 9 && co == SW_CO && ci >= 1 && ci <= 16; }
 
-static int small_wgrad_split(size_t P) { return (int)std::min<size_t>(148, std::max<size_t>(1, P / 512)); }
+static int small_wgrad_split(size_t P) { return (int)std::min<size_t>(NUM_SMS, std::max<size_t>(1, P / 512)); }
 
 size_t conv_small_wgrad_workspace_floats(int taps, int ci, int co, size_t P) {
     return (size_t)small_wgrad_split(P) * taps * ci * co;

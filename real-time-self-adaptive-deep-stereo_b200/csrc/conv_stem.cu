@@ -2,10 +2,9 @@
 // (reference Nets/DispNet.py:82-86 through sharedLayers.conv2d, Nets/sharedLayers.py:54-63) -- forward and the filter
 // gradient tf.gradients derives for it in the FULL train op (Stereo_Online_Adaptation.py:118,143-151).
 //
-// 2.3 GMAC per pass over 2 x 384 x 1280 pixels with a reduction depth of 3 channels: on the swap-AB tcgen05 path the K
-// block of every tap is 3 real channels in 32 (forward 301 us) and the weight gradient fills 3 of the 128 accumulator
-// lanes (1129 us, a quarter of the DispNet backward).  The CUDA cores do the same arithmetic in about 2.3 G FMAs / (148 SMs
-// x 128 lanes x 1.9 GHz) = 64 us; what decides is operand reuse in registers:
+// 2.3 GMAC per pass over 2 x 384 x 1280 pixels with a reduction depth of 3 channels: on the swap-AB tensor-core path the
+// K block of every tap is 3 real channels in 32 and the weight gradient fills 3 of the 128 accumulator rows.  The CUDA
+// cores do the same arithmetic without that padding; what decides is operand reuse in registers:
 //   wgrad  : a CTA stages an 8 x 16 output tile (input patch 21 x 37 x 3, dY 128 x 64) in shared memory; a thread owns
 //            5 (tap, ci) pairs x 8 output channels = 40 partial sums and reads 5 x + 8 dY values per 40 FMAs; CTAs are
 //            persistent over tiles and leave one partial vector each, folded in a fixed order (deterministic).
@@ -136,7 +135,7 @@ __global__ void conv_stem_wgrad_reduce_kernel(const float* __restrict__ part, in
 
 static int stem_wgrad_grid(const ConvWgrad& q) {
     const long ntiles = (long)q.dy.n * cdiv(q.dy.w, ST_TW) * cdiv(q.dy.h, ST_TH);
-    return (int)std::min<long>(ntiles, 2 * 148);
+    return (int)std::min<long>(ntiles, 2 * NUM_SMS);
 }
 bool conv_stem_wgrad_supported(const ConvWgrad& q) {
     return stem_geom(q.x.c, q.x.cs, q.dy.c, q.kh, q.kw, q.stride, q.dil) && q.x.n == q.dy.n && (q.dy.cs & 3) == 0 &&
@@ -198,7 +197,7 @@ conv_stem_fwd_kernel(ConvGemm g, int tiles_x, int tiles_y, unsigned short* __res
     // thread: 8 output channels (cq) of 4 horizontally adjacent output pixels (pg): 32 pixel groups x 8 channel groups.
     // Per filter row the 13 input pixels the 4 outputs touch (columns 2*px0 ... 2*px0 + 12) sit in registers and serve all
     // 7 horizontal taps: 13 + 42 128-bit shared loads per 672 FMAs.  (First version: 2 pixels x 16 channels, 6 loads per
-    // 32 FMAs -- 300 us, shared-memory bound.)
+    // 32 FMAs -- shared-memory bound.)
     const int cq = threadIdx.x & 7, pg = threadIdx.x >> 3;
     const int py = pg / (ST_TW / 4), px = (pg % (ST_TW / 4)) * 4;
     float acc[4][8];

@@ -289,8 +289,7 @@ __global__ void __launch_bounds__(CORR_NT) corr_fwd2_kernel(CorrFwd p, int TW, i
 }
 
 // ---------------------------------------------------------------------------------------------
-// forward v3: ncu on v2 (profiles/r1_ncu_corr_fwd2_L2_1920x1088_B8.txt) showed the kernel instruction-issue bound
-// (155 M warp instructions for 1.04 M pixels, 66 % issue-active, DRAM 16 %): with 8 lanes per pixel every lane owns a
+// forward v3: v2 is instruction-issue bound: with 8 lanes per pixel every lane owns a
 // single float4 chunk, so address arithmetic and the shuffle reductions dominate.  Here LP = 1..8 lanes share a pixel
 // and each lane owns CPL >= 3 consecutive chunks; the left chunk is held in registers across the nd displacements;
 // shared-memory tiles are stored with an XOR swizzle of the chunk index (low 3 bits ^ column&7) so that lane=column
@@ -472,7 +471,7 @@ int corr_fwd(const CorrFwd& p, cudaStream_t st) {
     if (ver >= 3) {
         const int nchunk = p.C / 4;
         const int LP = nchunk >= 24 ? 8 : (nchunk >= 16 ? 4 : (nchunk >= 8 ? 2 : 1));
-        // measured (scripts/corr_bench.py): v3 wins for C<=32 (level 2, which moves most of the bytes), v2 for wider features / nd=81
+        // v3 for C<=32 (level 2, which moves most of the bytes), v2 for wider features / nd=81
         if (nchunk % LP == 0 && p.C <= 32 && nd <= 8) {
             const int TW = std::min(p.w, CORR_NT / LP);
             const int RCAP = warped ? TW + 2 * p.max_disp + 32 : 0;

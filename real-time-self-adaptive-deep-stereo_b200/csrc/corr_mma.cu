@@ -6,13 +6,13 @@
 //     corr[b,y,x,i] = (1/C) * sum_c L[b,y,x,c] * R[b,y,x+i-D,c]          0 <= i <= 2D, zero outside the row
 // For one image row this is the band |x' - x| <= D of the w x w matrix L R^T.  The narrow-window kernels (corr.cu,
 // corr_tma.cu: 5 displacements) keep one pixel per 8 lanes and are bandwidth-shaped; at 81 displacements the same loop is
-// arithmetic-bound on the CUDA cores (0.64 GFLOP of scalar FMAs with one shared-memory operand each: 141 us at 1280x384,
+// arithmetic-bound on the CUDA cores (0.64 GFLOP of scalar FMAs with one shared-memory operand each at 1280x384,
 // 4.4 % of the HBM roofline).  Here a warp owns a 16-pixel block of x and the 16 + 2D window of x' it can reach:
 // 12 m16n8k16 tiles per K step for D = 40, 84 % of the multiplied entries inside the band.
 //
-// Why mma.sync and not tcgen05: the result has to be read along DIAGONALS (i = x' - x + D).  In the mma.sync accumulator
-// fragment a thread owns fixed (row, column) pairs, so i = col - row is a per-register constant and the band is extracted
-// with no data movement; a TMEM accumulator is read lane = row, so every lane would need a different column window.
+// Why mma.sync: the result has to be read along DIAGONALS (i = x' - x + D).  In the mma.sync accumulator fragment a
+// thread owns fixed (row, column) pairs, so i = col - row is a per-register constant and the band is extracted with no
+// data movement.
 // The op is 2 GFLOP of issued MMAs against 41 MB of HBM traffic -- the HBM roofline, not the tensor pipe, is the bound.
 //
 // Arithmetic: fp32 features are split while they are staged into shared memory, x * s = hi + lo in fp16 (22 mantissa

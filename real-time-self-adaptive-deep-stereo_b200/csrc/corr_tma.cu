@@ -4,9 +4,9 @@
 // Nets/MadNet.py:400-436 linear warp; native launcher Nets/Native/shift_corr.cu.cc:193-233), specialised for the MADNet
 // cost volume: max_disp = 2, stride 1 (5 displacements), C a multiple of 32.
 //
-// ncu on v3 (profiles/r1_ncu_corr_fwd3_L2_1920x1088_B8.txt) showed ~3000 thread instructions per pixel: staging loops
+// v3 (corr.cu) spends ~3000 thread instructions per pixel: staging loops
 // (index division, swizzle, 64-bit address math), bounds predicates in the inner loop and shuffle reductions, i.e. the
-// kernel was instruction-issue bound at 28 % of HBM.  Here
+// kernel is instruction-issue bound.  Here
 //   * the left tile, the right window and the left half of the concat buffer move by TMA tensor copies
 //     (cp.async.bulk.tensor, SWIZZLE_128B: a pixel's 32-channel block is one 128-byte row, its 16-byte chunks XOR-ed
 //     with row&7), so staging and the concat copy cost no thread instructions and reads are bank-conflict free with
@@ -278,7 +278,7 @@ int corr_fwd4(const CorrFwd& p, cudaStream_t st) {
     }
     const int LP = lp_env == 1 ? 1 : 2;
     const int ncb = p.C / 32;
-    // measured (profiles/r1_corr_v4_ab.log): 64-pixel tiles (7 CTAs per SM at C=32) beat 128; slack 16 beats 32
+    // 64-pixel tiles (7 CTAs per SM at C=32) rather than 128; slack 16 rather than 32
     int TW = tw_env > 0 ? tw_env : std::max(32, std::min(64, (128 / ncb + 7) / 8 * 8));
     TW = std::min(TW, 256 / LP);
     TW = std::min(TW, (p.w + 7) / 8 * 8);

@@ -178,7 +178,7 @@ int Engine::dp_update(int group, float lr, float mu, cudaStream_t st) {
     if (group >= 0) { MS_REQUIRE(group < n_groups, "dp_update: bad group"); b = group_begin[group]; e = group_end[group]; }
     const size_t n = e - b;
     MS_REQUIRE((n & 3) == 0 && (b & 3) == 0 && n + 4 <= dp_cap_floats, "dp_update: range not 16-byte granular / too large");
-    const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>(cdivz(n / 4, 256), 148 * 2));
+    const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>(cdivz(n / 4, 256), NUM_SMS * 2));
     dp_pack_kernel<<<blocks, 256, 0, st>>>(dp_state, dp_world, dp_rank, Gr + b, n, scalars, dp_xbuf);
     DpPeers peers;
     memset(&peers, 0, sizeof peers);

@@ -243,7 +243,7 @@ __global__ void u8_to_f32_kernel(const uchar4* __restrict__ src, float4* __restr
 int u8_to_f32(const unsigned char* src, float* dst, size_t n, cudaStream_t st) {
     MS_REQUIRE((n & 3) == 0 && (reinterpret_cast<uintptr_t>(src) & 3) == 0, "u8_to_f32: size / alignment");
     const size_t n4 = n / 4;
-    launch_k(u8_to_f32_kernel, dim3((unsigned)std::min<size_t>(cdivz(n4, 256), 148 * 8)), dim3(256), 0, st, reinterpret_cast<const uchar4*>(src),
+    launch_k(u8_to_f32_kernel, dim3((unsigned)std::min<size_t>(cdivz(n4, 256), NUM_SMS * 8)), dim3(256), 0, st, reinterpret_cast<const uchar4*>(src),
                                                                                        reinterpret_cast<float4*>(dst), n4);
     return check_launch("u8_to_f32");
 }

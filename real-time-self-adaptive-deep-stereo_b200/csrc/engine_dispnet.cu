@@ -54,8 +54,8 @@ void Engine::layout_dispnet(Bump& A, size_t& max_wg, size_t& max_wt) {
         max_wg = std::max(max_wg, conv_wgrad_workspace_floats(L.kh * L.kw, L.cin, L.cout, pixels));
         max_wg = std::max(max_wg, conv_wgrad_workspace_floats(L.kh * L.kw, L.cout, L.cin, pixels));
         max_wt = std::max(max_wt, (size_t)L.kh * L.kw * L.cin * L.cout);
-        if (L.cout == 1) max_wg = std::max(max_wg, (size_t)2 * 148 * ((size_t)L.kh * L.kw * L.cin + 1));    // conv_head_wgrad partials
-        if (L.kh == 7 && L.cin == 3 && L.cout == 64) max_wg = std::max(max_wg, (size_t)2 * 148 * (147 * 64 + 64));   // conv_stem_wgrad partials
+        if (L.cout == 1) max_wg = std::max(max_wg, (size_t)2 * NUM_SMS * ((size_t)L.kh * L.kw * L.cin + 1));    // conv_head_wgrad partials
+        if (L.kh == 7 && L.cin == 3 && L.cout == 64) max_wg = std::max(max_wg, (size_t)2 * NUM_SMS * (147 * 64 + 64));   // conv_stem_wgrad partials
         if (conv_impl == 1 && !L.transposed && L.cin >= 3 && L.cout >= 16) {
             max_wg = std::max(max_wg, std::min<size_t>(wgrad_bf_workspace_floats(L.kh, L.kw, L.cin, L.cout), (size_t)48 << 20));
             wg_xp_halfs = std::max(wg_xp_halfs, pixels * L.stride * L.stride * (size_t)((L.cin + 7) / 8 * 8));
@@ -184,7 +184,7 @@ int Engine::deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, co
         prof_begin(CAT_CONV_WGRAD, st, li);
         int rc;
         if (dpl && use_bf_wgrad && wg_xp.hi && wgrad_bf_supported(q)) {
-            // tcgen05: "x" = dY planes, "dy" = a bf16 re-split of the layer's forward input (kind::f16 rejects f16 x bf16)
+            // "x" = dY planes, "dy" = a bf16 re-split of the layer's forward input (a wgmma takes one 16-bit element type)
             ActPlanes xb = wg_xp; xb.cs = (x.c + 7) / 8 * 8;
             MS_REQUIRE(x.pixels() * (size_t)xb.cs <= wg_xp_halfs, "deconv_bwd: wgrad scratch planes too small");
             rc = split_planes(x, xb, st);
@@ -204,7 +204,7 @@ int Engine::deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, co
         p.x = dpre; p.wmat = Wt + L.w_off; p.bias = nullptr; p.y = *dx; p.kh = L.kh; p.kw = L.kw;
         p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1;
         p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = dx_acc;
-        p.part = tc_part; p.part_floats = conv_tc_part_floats();
+        p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
         prof_begin(CAT_CONV_DGRAD, st, li);
         int rc;
         if (dpl && bfw[1][li].ok && conv_bf_supported(p)) {

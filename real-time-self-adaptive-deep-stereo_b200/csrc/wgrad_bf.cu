@@ -1,4 +1,4 @@
-// wgrad_bf: tcgen05 weight (+ bias) gradient of a convolution on split-bf16 operands, stride 1 or 2, any dilation.
+// wgrad_bf: wgmma weight (+ bias) gradient of a convolution on split-bf16 operands, stride 1 or 2, any dilation.
 //
 // Replaces the filter- and bias-gradient sub-graphs tf.gradients derives for tf.nn.conv2d / tf.nn.atrous_conv2d /
 // tf.nn.bias_add (reference Nets/sharedLayers.py:58-59,72-73) inside the train ops of
@@ -7,25 +7,25 @@
 //   dW[r][s][ci][co] = sum over output pixels p of  X[p * stride + offset(r, s)][ci] * dY[p][co]
 //   db[co]           = sum over output pixels p of  dY[p][co]
 //
-// Both operands already exist as bf16 hi / lo planes in NHWC (the forward activation planes conv_bf reads, and the
-// gradient planes the dgrad epilogue writes), i.e. with the GEMM's reduction index (pixels) as the SLOW index.  The
-// UMMA descriptors take that layout directly as "MN-major" operands: a TMA box {64 channels, 8 pixels, rows}
-// with SWIZZLE_128B is exactly the canonical MN-major SW128 tile ((8,n),(8,k)):((1,LBO),(8,SBO)) [uint128 units] with
-// SBO = 1024 B (8 pixels) and LBO = the distance between 64-channel blocks -- no transposes, no in-kernel splitting
-// (the round-1 kernel, wgrad_tc.cu, needs an NHWC->NCHW copy of dY and splits fp32 into tf32 halves in the main loop).
+// Both operands already exist as 16-bit hi / lo planes in NHWC (the forward activation planes conv_bf reads, and the
+// gradient planes the dgrad epilogue writes), i.e. with the GEMM's reduction index (pixels) as the SLOW index.  The wgmma
+// descriptors take that layout directly as "MN-major" operands: a TMA box {64 channels, 8 pixels, rows} with
+// SWIZZLE_128B is exactly the canonical MN-major SW128 tile ((8,n),(8,k)):((1,LBO),(8,SBO)) [uint128 units] with
+// SBO = 1024 B (8 pixels) and LBO = the distance between 64-channel blocks -- no transposes, no in-kernel splitting.
 //
-// GEMM per CTA: one filter COLUMN s (all kh taps of it: one TMEM accumulator per tap), one 128-row block of ci,
-// one block of BN output channels, one slice of the pixel tiles (split-K):
-//   M = ci (128 TMEM lanes), N = BN co, K = pixels in tiles of 8 x TH.
+// GEMM per CTA: one filter COLUMN s (all kh <= 3 taps of it: one register accumulator per tap), one 128-row block of ci
+// (two warpgroups of m64 wgmma), one block of WB_BN = 64 output channels, one slice of the pixel tiles (split-K):
+//   M = ci, N = co, K = pixels in tiles of 8 x TH.
 //   For stride 1 and small dilation the kh taps read ONE halo patch of X (TH + (kh-1)*dil rows; a tap is a row offset =
 //   a whole number of 1024-byte swizzle atoms = a different descriptor start address); otherwise one box per tap
 //   (stride 2 through TMA element strides).
-//   Three kind::f16 MMAs per K step: X_lo*dY_hi + X_hi*dY_lo + X_hi*dY_hi (~2^-16 relative product error).
+//   Three 16-bit MMAs per K step: X_lo*dY_hi + X_hi*dY_lo + X_hi*dY_hi (~2^-16 relative product error).
 //   Bias gradient: CTAs of column 0 / block 0 run two more MMAs per K step with an all-ones A tile -> db in one more
 //   accumulator (no separate reduction kernel over dY).
 // Partial sums [split][tap][ci][co] (+ [split][co]) go to the workspace; a fixed-order reduce finishes (deterministic).
 //
-// Warp roles (320 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2-9 = epilogue.
+// Warpgroup roles (384 threads): warpgroup 0 = TMA producer (one warp issues), warpgroups 1-2 = wgmma on ci [0, 64) /
+// [64, 128) of the block, then they store their partial sums straight from the accumulator registers.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <algorithm>
@@ -34,12 +34,15 @@
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma_ptx.cuh"
 
 namespace ms {
 
-constexpr int WB_THREADS = 320;
+constexpr int WB_THREADS = 384;
 constexpr int WB_MAX_KH = 7;
-constexpr uint32_t WB_ONES_BYTES = 4096;       // 2 channel blocks x 2 k-groups x 1024 B of bf16 1.0
+constexpr int WB_ACC_TAPS = 3;                 // filter rows per launch: 3 tap accumulators + the bias accumulator
+constexpr int WB_BN = 64;                      // output channels per CTA
+constexpr uint32_t WB_ONES_BYTES = 4096;       // 2 channel blocks x 2 k-groups x 1024 B of 1.0
 constexpr uint32_t WB_ATOM = 1024;             // one tile row: 8 pixels x 64 channels x 2 B
 
 struct WgradBfParams {
@@ -51,40 +54,24 @@ struct WgradBfParams {
     short box_dy[WB_MAX_KH];       // input-row origin of box b relative to y0 * sx
     short tap_row[WB_MAX_KH];      // first X-region row of tap r
     int pad_l, dil;
-    int ci, co, mblocks, nblocks, BN, xblk, dblk;
+    int ci, co, mblocks, nblocks, xblk;
     int nstages;
     uint32_t stage_bytes, x_plane_bytes, d_plane_bytes;
-    int tmem_cols;
     int with_bias;
-    int xfmt, dfmt;                // plane formats of X and dY (0 = bf16, 1 = fp16 of value / 16)
     float* part;                   // [split][tap][ci][co]
     float* bpart;                  // [split][co]
     int tap0, taps_total;          // this launch covers filter rows [tap0 / kw, tap0 / kw + kh) of a taps_total-tap filter
-    int debug;                     // MS_WB_DEBUG bit mask (diagnosis): 1 no MMAs, 2 no TMA loads, 4 main product only, 8 product-major issue order
 };
 
-__device__ __forceinline__ void wb_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-// MN-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start >> 4 | LBO (distance
-// between 64-element blocks along M/N) | SBO (distance between 8-row groups along K) | version 1 | layout_type 2.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_byte_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((smem_byte_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46) | (2ull << 61);
-}
-
+// BF: 1 = bf16 planes, 0 = fp16 planes (both operands share the format: a wgmma takes one A / B element type)
+template <int BF>
 __global__ void __launch_bounds__(WB_THREADS, 1)
 wgrad_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant__ CUtensorMap mapXl,
                 const __grid_constant__ CUtensorMap mapDh, const __grid_constant__ CUtensorMap mapDl,
                 const __grid_constant__ WgradBfParams p) {
     pdl_prologue();
     extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t full_bar[4], empty_bar[4], accum_bar;
-    __shared__ uint32_t tmem_slot;
+    __shared__ __align__(8) uint64_t full_bar[4], empty_bar[4];
 
     const int warp = uniform_warp_idx(), lane = threadIdx.x & 31;
     const uint32_t base = (s_addr(smem_dyn) + 1023u) & ~1023u;
@@ -97,33 +84,25 @@ wgrad_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant
     const int s = bx / p.mblocks;                       // filter column
     const int split = blockIdx.y;
     const int t0 = (int)(((long)split * p.ntiles) / p.splits), t1 = (int)(((long)(split + 1) * p.ntiles) / p.splits);
-    const int total = t1 - t0;
     const bool do_bias = p.with_bias && s == 0 && mb == 0;
 
     if (threadIdx.x == 0) {
-        for (int i = 0; i < p.nstages; ++i) { mb_init(&full_bar[i], 1); mb_init(&empty_bar[i], 1); }
-        mb_init(&accum_bar, 1);
+        // full: the producer's expect_tx arrival + the bytes; empty: one arrival per MMA warp (8)
+        for (int i = 0; i < p.nstages; ++i) { mb_init(&full_bar[i], 1); mb_init(&empty_bar[i], 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_addr(&tmem_slot)), "r"((uint32_t)p.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (warp >= 2) {                                    // the all-ones A tile of the bias-gradient MMAs
+    if (warp >= 4) {                                    // the all-ones A tile of the bias-gradient MMAs
         uint32_t* ones = reinterpret_cast<uint32_t*>(gbase);
-        const uint32_t one2 = p.dfmt == 0 ? 0x3F803F80u : 0x3C003C00u;      // 1.0 in the format of the dY planes
-        for (int i = threadIdx.x - 64; i < (int)(WB_ONES_BYTES / 4); i += WB_THREADS - 64) ones[i] = one2;
+        const uint32_t one2 = BF ? 0x3F803F80u : 0x3C003C00u;      // 1.0 in the format of the dY planes
+        for (int i = threadIdx.x - 128; i < (int)(WB_ONES_BYTES / 4); i += WB_THREADS - 128) ones[i] = one2;
         fence_async_smem();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_slot;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ================= TMA producer: warp-uniform loop, elected lane issues =================
-        const bool leader = elect_one();
-        if (total > 0) {
+        if (warp == 0) {
+            const bool leader = elect_one();
             int st = 0; uint32_t ph = 0;
             const int tiles_img = p.tiles_x * p.tiles_y;
             const int offx = s * p.dil - p.pad_l;
@@ -132,7 +111,6 @@ wgrad_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant
                 const int rem = t - img * tiles_img;
                 const int ty = rem / p.tiles_x, tx = rem - ty * p.tiles_x;
                 mb_wait(&empty_bar[st], ph ^ 1u);
-                if (p.debug & 2) { if (leader) mb_arrive(&full_bar[st]); if (++st == p.nstages) { st = 0; ph ^= 1u; } continue; }
                 if (leader) mb_expect_tx(&full_bar[st], p.stage_bytes);
                 unsigned char* dst = gbase + stage0 + (size_t)st * p.stage_bytes;
                 for (int pl = 0; pl < 2 && leader; ++pl) {
@@ -144,143 +122,104 @@ wgrad_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant
                                         mb * 128 + b * 64, tx * 8 * p.sx + offx, ty * p.TH * p.sx + p.box_dy[q], img);
                     const CUtensorMap* md = pl ? &mapDl : &mapDh;
                     unsigned char* dd = dst + 2 * (size_t)p.x_plane_bytes + (size_t)pl * p.d_plane_bytes;
-                    for (int b = 0; b < p.dblk; ++b)
-                        tma_load_4d(dd + (size_t)(b * p.TH) * WB_ATOM, md, &full_bar[st], nb * p.BN + b * 64, tx * 8, ty * p.TH, img);
+                    tma_load_4d(dd, md, &full_bar[st], nb * WB_BN, tx * 8, ty * p.TH, img);
                 }
                 if (++st == p.nstages) { st = 0; ph ^= 1u; }
             }
         }
-    } else if (warp == 1) {
-        // ================= MMA issuer: warp-uniform loop, one elected lane issues (tc_ptx.cuh:elect_one) =================
-        const bool leader = elect_one();
-        const uint32_t tmem = __shfl_sync(0xffffffffu, tmem_slot, 0);
-        if (total > 0) {
-            // D = f32, A = B = bf16, both MN-major (bits 15, 16), N >> 3 at bit 17, M >> 4 at bit 24
-            // A (= X) / B (= dY) element formats follow the planes: 0 = f16, 1 = bf16 in the descriptor
-            const uint32_t fa = p.xfmt == 0 ? 1u : 0u, fb = p.dfmt == 0 ? 1u : 0u;
-            const uint32_t idesc = (1u << 4) | (fa << 7) | (fb << 10) | (1u << 15) | (1u << 16) |
-                                   ((uint32_t)(p.BN >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t idesc_ones = (1u << 4) | (fb << 7) | (fb << 10) | (1u << 15) | (1u << 16) |
-                                        ((uint32_t)(p.BN >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t lbo_x = p.xblk > 1 ? (uint32_t)p.x_rows * WB_ATOM : 0u;
-            const uint32_t lbo_d = (uint32_t)p.TH * WB_ATOM;
-            const uint64_t ones = umma_desc_mn_sw128(base, 2048u, 1024u);
-            const uint32_t acc_bias = tmem + (uint32_t)(p.kh * p.BN);
-            int st = 0; uint32_t ph = 0;
-            uint32_t started = 0;
-            const int ksteps = p.TH >> 1;
-            for (int t = t0; t < t1; ++t) {
-                mb_wait(&full_bar[st], ph);
-                tc_fence_after();
-                const uint32_t sb = base + stage0 + (uint32_t)st * p.stage_bytes;
-                const uint32_t xh = sb, xl = sb + p.x_plane_bytes;
-                const uint32_t dh = sb + 2u * p.x_plane_bytes, dl = dh + p.d_plane_bytes;
-                for (int j = 0; j < ((p.debug & 1) ? 0 : ksteps); ++j) {
-                    const uint64_t bh = umma_desc_mn_sw128(dh + (uint32_t)(2 * j) * WB_ATOM, lbo_d, 1024u);
-                    const uint64_t bl = umma_desc_mn_sw128(dl + (uint32_t)(2 * j) * WB_ATOM, lbo_d, 1024u);
-                    if (p.debug & 12) {                 // diagnosis variants: main product only (4) / product-major order (8)
-                        for (int pr = (p.debug & 4) ? 2 : 0; pr < 3; ++pr)
-                            for (int r = 0; r < p.kh; ++r) {
-                                const uint32_t ro = (uint32_t)(p.tap_row[r] + 2 * j) * WB_ATOM;
-                                const uint64_t ah = umma_desc_mn_sw128(xh + ro, lbo_x, 1024u);
-                                const uint64_t al = umma_desc_mn_sw128(xl + ro, lbo_x, 1024u);
-                                const uint32_t acc = tmem + (uint32_t)(r * p.BN);
-                                const bool first = pr == ((p.debug & 4) ? 2 : 0);
-                                if (leader) wb_mma_f16(acc, pr == 0 ? al : ah, pr == 1 ? bl : bh, idesc, first ? started : 1u);
-                            }
-                        started = 1u;
-                        continue;
-                    }
-                    for (int r = 0; r < p.kh; ++r) {
+        return;
+    }
+
+    // ================= MMA warpgroups: ci rows [64 * mg, 64 * mg + 64) of the block =================
+    const int mg = (warp >> 2) - 1;
+    const bool rows_live = mg < p.xblk;                 // (ci <= 64: the second warpgroup has no rows, only the bias MMAs run)
+    const bool bias_here = do_bias && mg == 0;
+    float acc[WB_ACC_TAPS][WB_BN / 2], accb[WB_BN / 2];
+#pragma unroll
+    for (int i = 0; i < WB_BN / 2; ++i) {
+        accb[i] = 0.f;
+#pragma unroll
+        for (int r = 0; r < WB_ACC_TAPS; ++r) acc[r][i] = 0.f;
+    }
+    {
+        const uint32_t x_rows_bytes = (uint32_t)p.x_rows * WB_ATOM;
+        const uint64_t ones = wg_desc(base, 2048u, 1024u, true);
+        int st = 0; uint32_t ph = 0;
+        int pend = -1;                                  // ring stage read by the MMAs still in flight
+        const int ksteps = p.TH >> 1;
+        for (int t = t0; t < t1; ++t) {
+            mb_wait(&full_bar[st], ph);
+            const uint32_t sb = base + stage0 + (uint32_t)st * p.stage_bytes;
+            const uint32_t xh = sb + (uint32_t)mg * x_rows_bytes, xl = xh + p.x_plane_bytes;
+            const uint32_t dh = sb + 2u * p.x_plane_bytes, dl = dh + p.d_plane_bytes;
+#pragma unroll
+            for (int r = 0; r < WB_ACC_TAPS; ++r) wg_fence_acc(acc[r]);
+            wg_fence_acc(accb);
+            wg_fence();
+            for (int j = 0; j < ksteps; ++j) {          // K = 16 pixels = two 8-pixel atoms
+                const uint64_t bh = wg_desc(dh + (uint32_t)(2 * j) * WB_ATOM, 0u, 1024u, true);
+                const uint64_t bl = wg_desc(dl + (uint32_t)(2 * j) * WB_ATOM, 0u, 1024u, true);
+                if (rows_live) {
+#pragma unroll
+                    for (int r = 0; r < WB_ACC_TAPS; ++r) {
+                        if (r >= p.kh) break;
                         const uint32_t ro = (uint32_t)(p.tap_row[r] + 2 * j) * WB_ATOM;
-                        const uint64_t ah = umma_desc_mn_sw128(xh + ro, lbo_x, 1024u);
-                        const uint64_t al = umma_desc_mn_sw128(xl + ro, lbo_x, 1024u);
-                        const uint32_t acc = tmem + (uint32_t)(r * p.BN);
-                        if (leader) {
-                            wb_mma_f16(acc, al, bh, idesc, started);
-                            wb_mma_f16(acc, ah, bl, idesc, 1u);
-                            wb_mma_f16(acc, ah, bh, idesc, 1u);
-                        }
+                        const uint64_t ah = wg_desc(xh + ro, 0u, 1024u, true);
+                        const uint64_t al = wg_desc(xl + ro, 0u, 1024u, true);
+                        Wgmma<WB_BN, BF, 1, 1>::mma(acc[r], al, bh);
+                        Wgmma<WB_BN, BF, 1, 1>::mma(acc[r], ah, bl);
+                        Wgmma<WB_BN, BF, 1, 1>::mma(acc[r], ah, bh);
                     }
-                    if (do_bias && leader) {
-                        wb_mma_f16(acc_bias, ones, bl, idesc_ones, started);
-                        wb_mma_f16(acc_bias, ones, bh, idesc_ones, 1u);
-                    }
-                    started = 1u;
                 }
-                if (leader) tc_commit(&empty_bar[st]);
-                if (++st == p.nstages) { st = 0; ph ^= 1u; }
+                if (bias_here) {
+                    Wgmma<WB_BN, BF, 1, 1>::mma(accb, ones, bl);
+                    Wgmma<WB_BN, BF, 1, 1>::mma(accb, ones, bh);
+                }
             }
-            if (leader) tc_commit(&accum_bar);
-            __syncwarp();
-        }
-    } else {
-        // ================= epilogue (warps 2..9): thread <-> ci row, columns <-> (tap, co) =================
-        const int q = warp & 3;                          // TMEM lane quarter this warp may access
-        const int half = (warp - 2) >> 2;
-        const int m = q * 32 + lane;
-        const int ci_g = mb * 128 + m;
-        const bool valid = ci_g < p.ci;
-        const uint32_t lane_base = (uint32_t)(q * 32) << 16;
-        if (total > 0) {
-            mb_wait(&accum_bar, 0);
-            tc_fence_after();
-        }
-        const int cpt = p.BN >> 4;                       // 16-column chunks per tap
-        const int chunks = p.kh * cpt;
-        const int cb = half ? (chunks + 1) / 2 : 0, ce = half ? chunks : (chunks + 1) / 2;
-        const bool vec = (p.co & 3) == 0;
-        const int taps = p.taps_total;
-        for (int c = cb; c < ce; ++c) {
-            const int r = c / cpt, c0 = (c - r * cpt) * 16;
-            uint32_t v[16];
-            if (total > 0) {
-                tc_ld16_nowait(tmem + lane_base + (uint32_t)(r * p.BN + c0), v);
-                tc_wait_ld();
-            } else {
+            wg_commit();
+            wg_wait<1>();                               // the previous stage's MMAs are done with their operands
 #pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = 0u;
-            }
-            if (!valid) continue;
+            for (int r = 0; r < WB_ACC_TAPS; ++r) wg_fence_acc(acc[r]);
+            wg_fence_acc(accb);
+            if (pend >= 0 && lane == 0) mb_arrive(&empty_bar[pend]);
+            pend = st;
+            if (++st == p.nstages) { st = 0; ph ^= 1u; }
+        }
+        wg_wait<0>();
+#pragma unroll
+        for (int r = 0; r < WB_ACC_TAPS; ++r) wg_fence_acc(acc[r]);
+        wg_fence_acc(accb);
+    }
+
+    // ================= partial sums straight from the fragments: (ci row, co pair) per register pair =================
+    const int wr = (warp & 3) * 16 + (lane >> 2);       // fragment row (+8 for the second half)
+    const int cc = 2 * (lane & 3);                      // fragment column (+8 j)
+    const int taps = p.taps_total;
+    if (rows_live) {
+#pragma unroll
+        for (int r = 0; r < WB_ACC_TAPS; ++r) {
+            if (r >= p.kh) break;
             const int tap = p.tap0 + r * p.kw + s;
-            const int co0 = nb * p.BN + c0;
-            float* prow = p.part + (((size_t)split * taps + tap) * p.ci + ci_g) * p.co + co0;
-            if (vec && co0 + 16 <= p.co) {
 #pragma unroll
-                for (int j = 0; j < 16; j += 4)
-                    *reinterpret_cast<float4*>(prow + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                        __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            } else {
+            for (int h = 0; h < 2; ++h) {
+                const int ci_g = mb * 128 + mg * 64 + wr + 8 * h;
+                if (ci_g >= p.ci) continue;
+                float* prow = p.part + (((size_t)split * taps + tap) * p.ci + ci_g) * p.co;
 #pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (co0 + j < p.co) prow[j] = __uint_as_float(v[j]);
-            }
-        }
-        if (do_bias && warp == 4) {                      // warp 4: lane quarter 0, row 0 holds sum_p dY[p][co]
-            for (int c0 = 0; c0 < p.BN; c0 += 16) {
-                uint32_t v[16];
-                if (total > 0) {
-                    tc_ld16_nowait(tmem + (uint32_t)(p.kh * p.BN + c0), v);
-                    tc_wait_ld();
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = 0u;
-                }
-                if (lane == 0) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int co = nb * p.BN + c0 + j;
-                        if (co < p.co) p.bpart[(size_t)split * p.co + co] = __uint_as_float(v[j]);
-                    }
+                for (int j = 0; j < WB_BN / 8; ++j) {
+                    const int co = nb * WB_BN + 8 * j + cc;
+                    if (co < p.co)      // (co is a multiple of 4 and cc even: the pair is whole)
+                        *reinterpret_cast<float2*>(prow + co) = make_float2(acc[r][4 * j + 2 * h], acc[r][4 * j + 2 * h + 1]);
                 }
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols) : "memory");
+    if (bias_here && (warp & 3) == 0 && (lane >> 2) == 0) {      // fragment row 0 holds sum_p dY[p][co]
+#pragma unroll
+        for (int j = 0; j < WB_BN / 8; ++j) {
+            const int co = nb * WB_BN + 8 * j + cc;
+            if (co < p.co) *reinterpret_cast<float2*>(p.bpart + (size_t)split * p.co + co) = make_float2(accb[4 * j], accb[4 * j + 1]);
+        }
     }
 }
 
@@ -312,7 +251,7 @@ __global__ void wgrad_bf_reduce_kernel(const float* __restrict__ part, float* __
 }
 
 struct WbPlan {
-    int TH, nbox, box_rows, x_rows, nstages, nblocks, BN, mblocks, xblk, dblk, splits, tiles_x, tiles_y, ntiles, tmem_cols;
+    int TH, nbox, box_rows, x_rows, nstages, nblocks, mblocks, xblk, splits, tiles_x, tiles_y, ntiles;
     uint32_t stage_bytes, x_plane_bytes, d_plane_bytes;
     bool ok;
 };
@@ -325,19 +264,9 @@ static WbPlan wb_plan(const ConvWgrad& q) {
     if (kh > WB_MAX_KH || kh * kw > 49) return P;
     if (ci < 3 || co < 16 || (co & 3)) return P;
     if ((size_t)q.dy.h * q.dy.w < 32) return P;
-    // output-channel blocks: (kh taps + bias) accumulators of BN columns in 512 TMEM columns
-    int nbk = 1, BN = 0;
-    for (;; ++nbk) {
-        BN = ((co + nbk - 1) / nbk + 15) / 16 * 16;
-        if ((kh + 1) * BN <= 512 && BN <= 256) break;
-        if (nbk > 16) return P;
-    }
-    P.nblocks = nbk; P.BN = BN;
+    P.nblocks = cdiv(co, WB_BN);
     P.mblocks = (ci + 127) / 128;
     P.xblk = ci > 64 ? 2 : 1;
-    P.dblk = (BN + 63) / 64;
-    const int need = (kh + 1) * BN;
-    P.tmem_cols = need <= 32 ? 32 : (need <= 64 ? 64 : (need <= 128 ? 128 : (need <= 256 ? 256 : 512)));
     const size_t budget = 222 * 1024 - WB_ONES_BYTES;
     const int cand[4] = {16, 8, 4, 2};
     for (int i = 0; i < 4; ++i) {
@@ -350,7 +279,7 @@ static WbPlan wb_plan(const ConvWgrad& q) {
         const int nbox = shared ? 1 : (parity ? 2 : kh);
         const int box_rows = shared ? TH + halo : (parity ? TH + (kh - 1) / 2 : TH);
         const int x_rows = nbox * box_rows;
-        const size_t xpb = (size_t)P.xblk * x_rows * WB_ATOM, dpb = (size_t)P.dblk * TH * WB_ATOM;
+        const size_t xpb = (size_t)P.xblk * x_rows * WB_ATOM, dpb = (size_t)TH * WB_ATOM;
         const size_t stage = 2 * (xpb + dpb);
         const int ns = (int)std::min<size_t>(4, budget / stage);
         if (ns < 2 || (ns < 3 && TH > 2)) continue;
@@ -364,7 +293,7 @@ static WbPlan wb_plan(const ConvWgrad& q) {
     P.tiles_x = cdiv(q.dy.w, 8); P.tiles_y = cdiv(q.dy.h, P.TH);
     P.ntiles = q.dy.n * P.tiles_x * P.tiles_y;
     const int cols = kw * P.mblocks * P.nblocks;
-    int splits = std::max(1, (148 + cols / 2) / cols);
+    int splits = std::max(1, (NUM_SMS + cols / 2) / cols);
     splits = std::min(splits, std::min(P.ntiles, 64));
     // bound the number of accumulation steps per CTA (the tensor core adds into fp32 with truncation)
     const int max_tiles = std::max(1, 8192 / (8 * P.TH));
@@ -382,7 +311,8 @@ size_t wgrad_bf_workspace_floats(int kh, int kw, int ci, int co) {
 int wgrad_bf_init() {
     static bool done = false;
     if (done) return 0;
-    MS_CHECK_CUDA(cudaFuncSetAttribute(wgrad_bf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    MS_CHECK_CUDA(cudaFuncSetAttribute(wgrad_bf_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    MS_CHECK_CUDA(cudaFuncSetAttribute(wgrad_bf_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     done = true;
     return 0;
 }
@@ -400,7 +330,8 @@ static int wgrad_bf_launch(const ConvWgrad& q, const ActPlanes& xp, const ActPla
         if (splits_force > 0) P.splits = std::max(1, std::min(splits_force, P.ntiles));
         MS_REQUIRE(splits_force <= 0 || P.splits == splits_force, "wgrad_bf: row groups disagree on the split factor");
     }
-    MS_REQUIRE(xp.fmt == dp.fmt, "wgrad_bf: tcgen05 kind::f16 rejects mixed f16 x bf16 operands (probed: illegal instruction); both plane sets must share a format");
+    MS_REQUIRE(xp.fmt == dp.fmt, "wgrad_bf: a wgmma takes one 16-bit element type; both plane sets must share a format");
+    MS_REQUIRE(q.kh <= WB_ACC_TAPS, "wgrad_bf: more filter rows than accumulators in one launch");
     MS_REQUIRE(xp.hi && xp.lo && dp.hi && dp.lo && (xp.cs & 7) == 0 && (dp.cs & 7) == 0 && xp.cs >= q.x.c && dp.cs >= q.dy.c,
                "wgrad_bf: operand planes missing");
     if (wgrad_bf_init()) return -1;
@@ -424,14 +355,11 @@ static int wgrad_bf_launch(const ConvWgrad& q, const ActPlanes& xp, const ActPla
     if (P.nbox == 1) p.box_dy[0] = (short)(-q.pad_t);
     if (parity) { p.box_dy[0] = (short)(-q.pad_t); p.box_dy[1] = (short)(1 - q.pad_t); }
     p.pad_l = q.pad_l; p.dil = q.dil;
-    p.ci = ci; p.co = co; p.mblocks = P.mblocks; p.nblocks = P.nblocks; p.BN = P.BN; p.xblk = P.xblk; p.dblk = P.dblk;
+    p.ci = ci; p.co = co; p.mblocks = P.mblocks; p.nblocks = P.nblocks; p.xblk = P.xblk;
     p.nstages = P.nstages; p.stage_bytes = P.stage_bytes; p.x_plane_bytes = P.x_plane_bytes; p.d_plane_bytes = P.d_plane_bytes;
-    p.tmem_cols = P.tmem_cols;
     p.with_bias = (q.db && r0 == 0) ? 1 : 0;
     p.tap0 = r0 * q.kw; p.taps_total = taps;
-    p.xfmt = xp.fmt; p.dfmt = dp.fmt;
     p.part = q.workspace;
-    { static int dbg = -1; if (dbg < 0) { const char* e = getenv("MS_WB_DEBUG"); dbg = e ? atoi(e) : 0; } p.debug = dbg; }
     p.bpart = q.workspace + (size_t)P.splits * wn;
 
     const CUtensorMap *mXh, *mXl, *mDh, *mDl;
@@ -452,23 +380,16 @@ static int wgrad_bf_launch(const ConvWgrad& q, const ActPlanes& xp, const ActPla
         if (bf_get_map(&mDl, dp.lo, 4, dims, strides, box, es, 128)) return -1;
     }
     const size_t smem = WB_ONES_BYTES + (size_t)P.nstages * P.stage_bytes + 1024;
-    launch_k(wgrad_bf_kernel, dim3(dim3(q.kw * P.mblocks * P.nblocks, P.splits)), dim3(WB_THREADS), smem, st, *mXh, *mXl, *mDh, *mDl, p);
+    const dim3 grid(q.kw * P.mblocks * P.nblocks, P.splits);
+    launch_k(xp.fmt == 0 ? wgrad_bf_kernel<1> : wgrad_bf_kernel<0>, grid, dim3(WB_THREADS), smem, st, *mXh, *mXl, *mDh, *mDl, p);
     if (splits_out) *splits_out = P.splits;
     return check_launch("wgrad_bf");
 }
 
-// Filter rows per launch.  Every filter row keeps its own accumulator (BN TMEM columns each, plus the bias row), so a tall
-// filter narrows BN: 5 rows leave 64 columns.  Measured (profiles/r2_wgrad_bf_killswitch.log, MMAs only, no loads):
-// 5 rows x BN 64 cost 200 cycles per MMA, 3 rows x BN 128 cost 119 -- per column three times dearer -- so filters with
-// 5 or more rows run as groups of <= 3 rows, each group its own launch with its own, shorter halo.
-static int wb_group_rows(const ConvWgrad& q) {
-    static int grp = -1;
-    if (grp < 0) { const char* e = getenv("MS_WB_GROUPS"); grp = (e && e[0] == '0') ? 0 : 1; }
-    // in the DispNet step graph (profiles/r2_layers_in_graph_cfg4.json vs r2_layers_cfg4_groups.json): 5 x 5 layers gain
-    // (conv2 462 -> 349 us, conv3 238 -> 152 us), the 4 x 4 transposed-conv gradients as 2 + 2 rows lose (36 -> 73 us)
-    if (!grp || q.kh <= 4) return q.kh;
-    return 3;
-}
+// Filter rows per launch.  Every filter row keeps its own register accumulator (WB_BN / 2 floats per thread, plus the bias
+// accumulator), so filters with more than WB_ACC_TAPS rows run as groups of at most that many rows, each group its own
+// launch with its own, shorter halo.
+static int wb_group_rows(const ConvWgrad& q) { return std::min(q.kh, WB_ACC_TAPS); }
 
 // xp / dp: bf16 planes of q.x / q.dy
 int wgrad_bf(const ConvWgrad& q, const ActPlanes& xp, const ActPlanes& dp, cudaStream_t st) {
@@ -508,92 +429,6 @@ int wgrad_bf(const ConvWgrad& q, const ActPlanes& xp, const ActPlanes& dp, cudaS
     launch_k(wgrad_bf_reduce_kernel, dim3((unsigned)cdivz(work, 256)), dim3(256), 0, st, p.part, q.dw, n4, P.splits, p.bpart, q.db, co, q.accumulate,
                                                                       sx16 * sd16, sd16);
     return check_launch("wgrad_bf_reduce", 1);
-}
-
-// ------------------------------------------------------------------------------------------------
-// tcgen05.mma cost probe (diagnosis, scripts/mma_probe.py): one CTA per SM, one thread issues `iters` back-to-back
-// kind::f16 MMAs (M = 128, K = 16, bf16) on zero-filled shared memory -- no loads, no epilogue -- and the cycles between the
-// first issue and the completion of the last one are reported per CTA.
-//   a_mn / b_mn : operand layout (0 = K-major SW128 as in conv_bf, 1 = MN-major SW128 as in wgrad_bf)
-//   n           : MMA N;   n_acc : accumulators visited round-robin (each n columns);  rot : 1 = rotate the operand
-//   addresses over 4 atoms like the real K loop, 0 = the same operands every time;  uni : issue scheme (see the kernel)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t probe_desc_k_sw128(uint32_t smem_byte_addr) {
-    return (uint64_t)((smem_byte_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__global__ void __launch_bounds__(128, 1) mma_probe_kernel(int a_mn, int b_mn, int n, int n_acc, int rot, int iters, int uni, long long* out) {
-    extern __shared__ unsigned char smem_dyn[];
-    __shared__ __align__(8) uint64_t bar;
-    __shared__ uint32_t tmem_slot;
-    const uint32_t base = (s_addr(smem_dyn) + 1023u) & ~1023u;
-    unsigned char* gbase = smem_dyn + (base - s_addr(smem_dyn));
-    for (int i = threadIdx.x; i < 96 * 1024 / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(gbase)[i] = 0u;
-    fence_async_smem();
-    if (threadIdx.x == 0) { mb_init(&bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (threadIdx.x < 32) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_addr(&tmem_slot)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const int warp = uniform_warp_idx();
-    // uni = 0: the loop runs on lane 0 only (round-2 kernels before this probe); uni = 1: on the whole warp, uniform control
-    // flow, the MMA itself predicated on an elected lane
-    if ((uni && warp == 0) || (!uni && threadIdx.x == 0)) {
-        const bool leader = uni ? elect_one() : true;
-        const uint32_t tmem = uni ? __shfl_sync(0xffffffffu, tmem_slot, 0) : tmem_slot;
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-                               ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-        const uint32_t a0 = base, b0 = base + 48 * 1024;
-        // operands and accumulators of 4 consecutive K steps, fixed before the loop: the loop body is 4 MMAs and a counter
-        // (the first version of this probe selected layouts, rotated addresses and took `i % n_acc` INSIDE the loop and
-        // measured its own 150 - 240 cycles of integer work per iteration, profiles/r2_mma_probe_lane0_loop.log)
-        uint64_t ad[4], bd[4];
-        uint32_t acc[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t step = rot ? (uint32_t)k : 0u;
-            ad[k] = a_mn ? umma_desc_mn_sw128(a0 + step * 2048u, 8u * 1024u, 1024u) : probe_desc_k_sw128(a0) + (uint64_t)(step * 2u);
-            bd[k] = b_mn ? umma_desc_mn_sw128(b0 + step * 2048u, 8u * 1024u, 1024u) : probe_desc_k_sw128(b0) + (uint64_t)(step * 2u);
-            acc[k] = tmem + (uint32_t)((k % n_acc) * n);
-        }
-        const long long t0 = clock64();
-        for (int i = 0; i < iters; i += 4) {
-            const uint32_t on = i ? 1u : 0u;
-            if (leader) {
-                wb_mma_f16(acc[0], ad[0], bd[0], idesc, on);
-                wb_mma_f16(acc[1], ad[1], bd[1], idesc, n_acc > 1 ? on : 1u);
-                wb_mma_f16(acc[2], ad[2], bd[2], idesc, n_acc > 2 ? on : 1u);
-                wb_mma_f16(acc[3], ad[3], bd[3], idesc, n_acc > 3 ? on : 1u);
-            }
-        }
-        const long long t1 = clock64();
-        if (leader) tc_commit(&bar);
-        mb_wait(&bar, 0);
-        const long long t2 = clock64();
-        if (leader) {
-            out[2 * blockIdx.x] = t1 - t0;          // issue loop
-            out[2 * blockIdx.x + 1] = t2 - t0;      // until the last MMA retired
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    }
-}
-int mma_probe(int a_mn, int b_mn, int n, int n_acc, int rot, int iters, int uni, int ctas, long long* out_dev, cudaStream_t st) {
-    MS_REQUIRE(n >= 16 && n <= 256 && (n & 15) == 0 && (n_acc == 1 || n_acc == 2 || n_acc == 4) && n_acc * n <= 512 && ctas >= 1 && (iters & 3) == 0,
-               "mma_probe: bad arguments");
-    static bool init = false;
-    if (!init) {
-        MS_CHECK_CUDA(cudaFuncSetAttribute(mma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-        init = true;
-    }
-    mma_probe_kernel<<<ctas, 128, 97 * 1024 + 1024, st>>>(a_mn, b_mn, n, n_acc, rot, iters, uni, out_dev);
-    return check_launch("mma_probe");
 }
 
 // one-shot convenience (operator-level C ABI / tests): splits x and dy into planes, runs the kernel.

@@ -1,4 +1,4 @@
-"""madstereo — Python host of the B200-native self-adaptive stereo engine (libmadstereo.so).
+"""madstereo — Python host of the H100-native self-adaptive stereo engine (libmadstereo.so).
 
 The public, reference-compatible API lives in the sibling packages `Nets`, `Sampler`, `Losses`,
 `Data_utils` (same module and function names as the reference repo); this package holds the ctypes

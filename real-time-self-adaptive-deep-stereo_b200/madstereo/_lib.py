@@ -24,14 +24,10 @@ _SIGS = {
     'ms_version': (I, []),
     'ms_last_error': (c_char_p, []),
     'ms_corr_fwd': (I, [P, I, P, I, P, I, P, I, I, I, I, I, I, I, I, I, P]),
-    'ms_debug_mma_probe': (I, [I, I, I, I, I, I, I, I, P, P]),
     'ms_corr_fwd_wide': (I, [P, I, P, I, P, I, I, I, I, I, I, F, P]),
     'ms_corr_bwd': (I, [P, I, P, I, P, I, P, I, P, I, P, I, P, I, I, I, I, I, I, I, I, P]),
     'ms_conv2d_fwd': (I, [P, I, I, I, I, I, P, P, P, I, I, I, I, I, I, F, P]),
     'ms_conv2d_dgrad': (I, [P, I, I, I, I, I, P, P, I, I, I, I, I, I, I, I, P, P]),
-    'ms_conv2d_fwd_tc': (I, [P, I, I, I, I, I, P, P, P, I, I, I, I, I, F, P, Z, P]),
-    'ms_conv2d_dgrad_tc': (I, [P, I, I, I, I, I, P, P, I, I, I, I, I, P, Z, P]),
-    'ms_conv2d_tc_scratch': (Z, [I, I, I, I]),
     'ms_conv2d_fwd_bf': (I, [P, I, I, I, I, I, P, P, P, I, I, I, I, I, I, F, F, P, Z, P]),
     'ms_conv2d_dgrad_bf': (I, [P, I, I, I, I, I, P, P, I, I, I, I, I, I, I, I, P, Z, P]),
     'ms_conv2d_bf_scratch': (Z, [I, I, I, I, I, I, I]),
@@ -45,8 +41,6 @@ _SIGS = {
     'ms_conv2d_bf_ticket_words': (Z, []),
     'ms_conv2d_wgrad_bf_planes': (I, [P, P, I, I, I, I, I, P, P, I, I, I, I, P, P, I, I, I, I, P, Z, P]),
     'ms_conv2d_wgrad_bf_workspace': (Z, [I, I, I, I]),
-    'ms_conv2d_wgrad_tc': (I, [P, I, I, I, I, I, P, I, I, P, P, I, I, I, P, Z, P]),
-    'ms_conv2d_wgrad_tc_workspace': (Z, [I, I, I, I, I, I, I]),
     'ms_conv2d_wgrad_workspace': (Z, [I, I, I, I, Z]),
     'ms_conv2d_wgrad': (I, [P, I, I, I, I, I, P, I, I, I, I, P, P, I, I, I, I, P, Z, P]),
     'ms_conv2d_transpose_fwd': (I, [P, I, I, I, I, I, P, P, P, I, I, I, I, I, F, P, P]),
@@ -94,8 +88,6 @@ _SIGS = {
     'ms_engine_profile_layers': (I, [P, P, P]),
     'ms_engine_profile_event_overhead_ms': (F, [P]),
     'ms_launch_count': (ctypes.c_longlong, []),
-    'ms_debug_tc_prof': (I, [POINTER(ctypes.c_ulonglong), I]),
-    'ms_debug_bf_prof': (I, [P, I]),
     'ms_engine_num_tensors': (I, [P]),
     'ms_engine_tensor_name': (I, [P, I, c_char_p, I]),
     'ms_engine_tensor': (I, [P, c_char_p, POINTER(P), POINTER(I)]),

@@ -103,31 +103,8 @@ def conv2d(x, w, b, stride=1, dilation=1, alpha=1.0):
     return y
 
 
-def conv2d_tc(x, w, b, dilation=1, alpha=1.0):
-    """tcgen05 / 3xTF32 forward of a stride-1 conv (same semantics as conv2d)."""
-    n, h, wd, cin = x.shape
-    kh, kw, _, cout = w.shape
-    y = torch.empty(n, h, wd, cout, device=x.device, dtype=torch.float32)
-    ns = lib().ms_conv2d_tc_scratch(kh, kw, cin, cout)
-    scratch = torch.empty(ns, device=x.device, dtype=torch.float32)
-    check(lib().ms_conv2d_fwd_tc(_p(x), n, h, wd, cin, cin, _p(w), _p(b), _p(y), cout, cout, kh, kw, dilation,
-                                 float(alpha), _p(scratch), ns, _s()), 'ms_conv2d_fwd_tc')
-    return y
-
-
-def conv2d_dgrad_tc(dy, w, dilation=1):
-    n, h, wd, cout = dy.shape
-    kh, kw, cin, _ = w.shape
-    dx = torch.empty(n, h, wd, cin, device=dy.device, dtype=torch.float32)
-    ns = lib().ms_conv2d_tc_scratch(kh, kw, cin, cout)
-    scratch = torch.empty(ns, device=dy.device, dtype=torch.float32)
-    check(lib().ms_conv2d_dgrad_tc(_p(dy), n, h, wd, cout, cout, _p(w), _p(dx), cin, cin, kh, kw, dilation,
-                                   _p(scratch), ns, _s()), 'ms_conv2d_dgrad_tc')
-    return dx
-
-
 def conv2d_bf(x, w, b, stride=1, dilation=1, alpha=1.0, act_scale=0.0625):
-    """split-bf16 tcgen05 forward conv (csrc/conv_bf.cu; same semantics as conv2d, stride 1 or 2)."""
+    """split-16-bit wgmma forward conv (csrc/conv_bf.cu; same semantics as conv2d, stride 1 or 2)."""
     n, h, wd, cin = x.shape
     kh, kw, _, cout = w.shape
     y = torch.empty(n, same_out(h, stride), same_out(wd, stride), cout, device=x.device, dtype=torch.float32)
@@ -153,7 +130,7 @@ def conv2d_dgrad_bf(dy, w, in_hw=None, stride=1, dilation=1):
 
 
 def conv2d_wgrad_bf(x, dy, kh, kw, stride=1, dilation=1):
-    """tcgen05 weight + bias gradient on bf16 hi/lo planes (csrc/wgrad_bf.cu), stride 1 or 2."""
+    """wgmma weight + bias gradient on bf16 hi/lo planes (csrc/wgrad_bf.cu), stride 1 or 2."""
     n, h, wd, cin = x.shape
     _, oh, ow, cout = dy.shape
     dw = torch.empty(kh, kw, cin, cout, device=x.device, dtype=torch.float32)
@@ -199,7 +176,7 @@ def _scratch256(nbytes, device):
 
 
 def conv2d_transpose_bf(x, w, b, stride=2, alpha=1.0, act_scale=0.0625):
-    """sharedLayers.conv2d_transpose on the tcgen05 path (fp16 hi/lo planes). w [kh,kw,cout,cin]."""
+    """sharedLayers.conv2d_transpose on the wgmma path (fp16 hi/lo planes). w [kh,kw,cout,cin]."""
     n, h, wd, cin = x.shape
     kh, kw, cout, _ = w.shape
     y = torch.empty(n, h * stride, wd * stride, cout, device=x.device, dtype=torch.float32)
@@ -211,7 +188,7 @@ def conv2d_transpose_bf(x, w, b, stride=2, alpha=1.0, act_scale=0.0625):
 
 
 def conv2d_transpose_dgrad_bf(dy, w, stride=2):
-    """d(conv2d_transpose)/dx on the tcgen05 path (bf16 hi/lo planes). dy [n,h*s,w*s,cout], w [kh,kw,cout,cin]."""
+    """d(conv2d_transpose)/dx on the wgmma path (bf16 hi/lo planes). dy [n,h*s,w*s,cout], w [kh,kw,cout,cin]."""
     n, oh, ow, cout = dy.shape
     kh, kw, _, cin = w.shape
     h, wd = oh // stride, ow // stride
@@ -224,7 +201,7 @@ def conv2d_transpose_dgrad_bf(dy, w, stride=2):
 
 
 def conv2d_transpose_wgrad_bf(x, dy, kh, kw, stride=2):
-    """d(conv2d_transpose)/dW [kh,kw,cout,cin] and /db [cout] on the tcgen05 path (bf16 hi/lo planes)."""
+    """d(conv2d_transpose)/dW [kh,kw,cout,cin] and /db [cout] on the wgmma path (bf16 hi/lo planes)."""
     n, h, wd, cin = x.shape
     cout = dy.shape[3]
     dw = torch.empty(kh, kw, cout, cin, device=x.device, dtype=torch.float32)
@@ -256,19 +233,6 @@ def conv2d_wgrad(x, dy, kh, kw, stride=1, dilation=1):
     ws = torch.empty(nws, device=x.device, dtype=torch.float32)
     check(lib().ms_conv2d_wgrad(_p(x), n, h, wd, cin, cin, _p(dy), oh, ow, cout, cout, _p(dw), _p(db), kh, kw,
                                 stride, dilation, _p(ws), nws, _s()), 'ms_conv2d_wgrad')
-    return dw, db
-
-
-def conv2d_wgrad_tc(x, dy, kh, kw, dilation=1):
-    """tcgen05 / 3xTF32 weight + bias gradient of a stride-1 conv."""
-    n, h, wd, cin = x.shape
-    cout = dy.shape[3]
-    dw = torch.empty(kh, kw, cin, cout, device=x.device, dtype=torch.float32)
-    db = torch.empty(cout, device=x.device, dtype=torch.float32)
-    nws = lib().ms_conv2d_wgrad_tc_workspace(kh, kw, cin, cout, n, h, wd)
-    ws = torch.empty(nws, device=x.device, dtype=torch.float32)
-    check(lib().ms_conv2d_wgrad_tc(_p(x), n, h, wd, cin, cin, _p(dy), cout, cout, _p(dw), _p(db), kh, kw, dilation,
-                                   _p(ws), nws, _s()), 'ms_conv2d_wgrad_tc')
     return dw, db
 
 
