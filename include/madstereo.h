@@ -192,7 +192,7 @@ int ms_engine_bind(void* e, float* weights, float* grads, float* momentum, float
 /* left/right: [B,H,W,3] fp32 0..255, host (pinned recommended) or device pointers. */
 int ms_engine_set_input(void* e, const float* left, const float* right, void* stream);
 /* the same with uint8 frames [B,H,W,3] (host or device): what the reference's decode ops deliver before tf.cast
- * (Data_utils/data_reader.py); converted to fp32 on the device. */
+ * (Data_utils/data_reader.py); converted to fp32 on the device.  Any B, H, W (B*H*W*3 need not be a multiple of 4). */
 int ms_engine_set_input_u8(void* e, const unsigned char* left, const unsigned char* right, void* stream);
 int ms_engine_set_gt(void* e, const float* gt, void* stream);
 /* Continual-adaptation variant (reference Stereo_Continual_Adaptation.py:75,112,133; Losses/loss_factory.py:304-351

@@ -232,19 +232,25 @@ int fill(float* p, size_t n, float v, cudaStream_t st) {
     return check_launch("fill");
 }
 
-// uint8 image -> fp32 (what tf.image.decode_* + tf.cast do in the reference input pipeline, Data_utils/data_reader.py)
-__global__ void u8_to_f32_kernel(const uchar4* __restrict__ src, float4* __restrict__ dst, size_t n4) {
+// uint8 image -> fp32 (what tf.image.decode_* + tf.cast do in the reference input pipeline, Data_utils/data_reader.py).
+// Four elements per uchar4 load; the last n % 4 elements (e.g. a 1242x375 KITTI frame: 1397250 bytes) are converted one
+// by one by the first threads of the grid.
+__global__ void u8_to_f32_kernel(const unsigned char* __restrict__ src, float* __restrict__ dst, size_t n) {
     pdl_prologue();
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-        const uchar4 v = src[i];
-        dst[i] = make_float4((float)v.x, (float)v.y, (float)v.z, (float)v.w);
+    const size_t n4 = n / 4;
+    const uchar4* s4 = reinterpret_cast<const uchar4*>(src);
+    float4* d4 = reinterpret_cast<float4*>(dst);
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (size_t i = t; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+        const uchar4 v = s4[i];
+        d4[i] = make_float4((float)v.x, (float)v.y, (float)v.z, (float)v.w);
     }
+    if (t < (n & 3)) dst[n4 * 4 + t] = (float)src[n4 * 4 + t];
 }
 int u8_to_f32(const unsigned char* src, float* dst, size_t n, cudaStream_t st) {
-    MS_REQUIRE((n & 3) == 0 && (reinterpret_cast<uintptr_t>(src) & 3) == 0, "u8_to_f32: size / alignment");
-    const size_t n4 = n / 4;
-    launch_k(u8_to_f32_kernel, dim3((unsigned)std::min<size_t>(cdivz(n4, 256), NUM_SMS * 8)), dim3(256), 0, st, reinterpret_cast<const uchar4*>(src),
-                                                                                       reinterpret_cast<float4*>(dst), n4);
+    MS_REQUIRE((reinterpret_cast<uintptr_t>(src) & 3) == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0, "u8_to_f32: alignment");
+    if (n == 0) return 0;
+    launch_k(u8_to_f32_kernel, dim3((unsigned)std::min<size_t>(cdivz(n / 4 + 1, 256), NUM_SMS * 8)), dim3(256), 0, st, src, dst, n);
     return check_launch("u8_to_f32");
 }
 

@@ -351,7 +351,7 @@ size_t Engine::layout(float* base) {
     rs_tmp_floats = (size_t)B * H * Wp; rs_tmp = alloc(rs_tmp_floats);
     loss_ws_floats = loss_workspace_floats(B, H, W); loss_ws = alloc(loss_ws_floats);
     scalars = alloc(64);
-    u8_stage = reinterpret_cast<unsigned char*>(alloc(((size_t)2 * B * H * W * 3 + 3) / 4 + 64));
+    u8_stage = reinterpret_cast<unsigned char*>(alloc((2 * u8_stage_right_offset((size_t)B * H * W * 3)) / 4 + 64));
     gt = alloc((size_t)B * H * W);
     proxy = alloc((size_t)B * H * W);
     return A.off;
@@ -516,16 +516,17 @@ int Engine::set_input(const float* left, const float* right, cudaStream_t st) {
     return 0;
 }
 
-// uint8 frames (host or device): 4x fewer bytes over PCIe than fp32; converted on the device
+// uint8 frames (host or device): 4x fewer bytes over PCIe than fp32; converted on the device.  Any B*H*W: the right frame
+// is staged at the next 4-byte boundary so that both halves are read with aligned uchar4 loads.
 int Engine::set_input_u8(const unsigned char* left, const unsigned char* right, cudaStream_t st) {
     MS_REQUIRE(bound, "engine not bound");
     TView rl = tensors["raw_left"], rr = tensors["raw_right"];
     const size_t n = (size_t)B * H * W * 3;
-    MS_REQUIRE((n & 3) == 0, "set_input_u8: B*H*W*3 must be a multiple of 4");
+    unsigned char* right_stage = u8_stage + u8_stage_right_offset(n);
     MS_CHECK_CUDA(cudaMemcpyAsync(u8_stage, left, n, cudaMemcpyDefault, st));
-    MS_CHECK_CUDA(cudaMemcpyAsync(u8_stage + n, right, n, cudaMemcpyDefault, st));
+    MS_CHECK_CUDA(cudaMemcpyAsync(right_stage, right, n, cudaMemcpyDefault, st));
     if (u8_to_f32(u8_stage, rl.p, n, st)) return -1;
-    return u8_to_f32(u8_stage + n, rr.p, n, st);
+    return u8_to_f32(right_stage, rr.p, n, st);
 }
 
 int Engine::prep_layers(int group, cudaStream_t st) {

@@ -36,6 +36,9 @@ struct Bump {            // workspace bump allocator (sizes only when base == nu
     TView tens(int n, int h, int w, int c, int cs = 0) { cs = cs ? cs : c; return view(alloc((size_t)n * h * w * cs), n, h, w, c, cs); }
 };
 
+// byte offset of the right frame in the uint8 staging buffer: the left frame's n bytes rounded up to 4
+inline size_t u8_stage_right_offset(size_t n) { return (n + 3) & ~(size_t)3; }
+
 struct Engine {
     // configuration
     int net;              // 0 = MADNet, 1 = DispNet

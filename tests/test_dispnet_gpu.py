@@ -29,11 +29,13 @@ def build(left, right, mode):
     return net, ad, params, lt, rt
 
 
-@pytest.mark.parametrize('hw', [(64, 128), (100, 200)])
+# (h, w) or (h, w, batch): batch 3 (odd, every frame seeded separately) compares every frame of the batched step
+@pytest.mark.parametrize('hw', [(64, 128), (100, 200), pytest.param((64, 128, 3), id='64x128-b3')])
 def test_dispnet_forward_parity(hw):
     from madstereo.synthetic import make_pair
     from oracle.dispnet import DispNetOracle
-    left, right, _ = make_pair(hw[0], hw[1], seed=5)
+    h, w, batch = (tuple(hw) + (1,))[:3]
+    left, right, _ = make_pair(h, w, seed=5, batch=batch)
     net, ad, params, lt, rt = build(left, right, 'NONE')
     assert len(net.get_disparities()) == 7
     names = list(net.get_layers_names())
@@ -53,9 +55,17 @@ def test_dispnet_forward_parity(hw):
 
 
 def test_dispnet_full_step_parity():
+    _check_full_step(batch=1)
+
+
+def test_dispnet_full_step_parity_batch3():
+    _check_full_step(batch=3)
+
+
+def _check_full_step(batch):
     from madstereo.synthetic import make_pair
     from oracle.dispnet import DispNetAdapter
-    left, right, _ = make_pair(64, 128, seed=5)
+    left, right, _ = make_pair(64, 128, seed=5, batch=batch)
     net, ad, params, lt, rt = build(left, right, 'FULL')
     orc = DispNetAdapter(params, mode='FULL', lr=1e-4)
     out = ad.step(lt, rt)

@@ -30,6 +30,16 @@ def rel_linf(a, b):
     return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-30))
 
 
+def hwb(shape):
+    """(h, w) or (h, w, batch) test parameter -> h, w, batch; make_pair(batch=B) seeds every frame separately."""
+    h, w, batch = (tuple(shape) + (1,))[:3]
+    return h, w, batch
+
+
+# batch 3 (odd, distinct frames): every frame of the batched engine step is compared with the oracle at batch 3
+B3 = pytest.param((64, 128, 3), id='64x128-b3')
+
+
 def build(left, right, mode, cfg='MadNet_full.json', **kw):
     import Nets
     from madstereo.adaptation import OnlineAdaptation
@@ -64,12 +74,12 @@ def test_api_surface():
         Nets.get_stereo_net('nope', {})
 
 
-@pytest.mark.parametrize('hw', [(64, 128), (128, 256), (100, 200)])
+@pytest.mark.parametrize('hw', [(64, 128), (128, 256), (100, 200), B3, pytest.param((100, 200, 3), id='100x200-b3')])
 def test_forward_parity(hw):
     from madstereo.synthetic import make_pair
     from oracle.madnet import MadNetOracle
-    h, w = hw
-    left, right, _ = make_pair(h, w, seed=3)
+    h, w, batch = hwb(hw)
+    left, right, _ = make_pair(h, w, seed=3, batch=batch)
     net, ad, params, lt, rt = build(left, right, 'NONE')
     eng = net.engine
     eng.set_input(lt, rt)
@@ -111,12 +121,12 @@ def test_forward_matches_golden_fixture(which):
 
 
 @pytest.mark.parametrize('module', [0, 1, 2, 3, 4])
-@pytest.mark.parametrize('hw', [(64, 128), (100, 200)])
+@pytest.mark.parametrize('hw', [(64, 128), (100, 200), B3])
 def test_mad_step_parity(module, hw):
     from madstereo.synthetic import make_pair
     from oracle.adaptation import OracleAdapter
-    h, w = hw
-    left, right, _ = make_pair(h, w, seed=3)
+    h, w, batch = hwb(hw)
+    left, right, _ = make_pair(h, w, seed=3, batch=batch)
     net, ad, params, lt, rt = build(left, right, 'MAD')
     ad.sampler._fixed_id = module
     orc = OracleAdapter(params, mode='MAD', lr=1e-4)
@@ -175,8 +185,11 @@ def test_mad_two_blocks_per_frame():
             assert np.array_equal(v, params[n]), n
 
 
-@pytest.mark.parametrize('mode,module', [('MAD', 1), ('MAD', 4), ('FULL', None)])
-def test_continual_proxy_loss_step(mode, module):
+@pytest.mark.parametrize('mode,module,batch', [pytest.param('MAD', 1, 1, id='MAD-1'), pytest.param('MAD', 4, 1, id='MAD-4'),
+                                               pytest.param('FULL', None, 1, id='FULL-None'),
+                                               pytest.param('MAD', 4, 3, id='MAD-4-b3'),
+                                               pytest.param('FULL', None, 3, id='FULL-None-b3')])
+def test_continual_proxy_loss_step(mode, module, batch):
     """SURVEY 8f-3: one adaptation step supervised by proxy disparities (Stereo_Continual_Adaptation.py:75,112,133;
     get_proxy_loss('mean_l1'), weights 0.01 / 0.1) against the oracle: losses, gradients, adapted weights; plus --dilation."""
     from madstereo.adaptation import OnlineAdaptation
@@ -184,10 +197,11 @@ def test_continual_proxy_loss_step(mode, module):
     from oracle.adaptation import OracleAdapter
     from oracle.madnet import init_params
     import Nets
-    left, right, gt = make_pair(64, 128, seed=3)
+    left, right, gt = make_pair(64, 128, seed=3, batch=batch)
     proxy = gt.copy()
     proxy[:, ::7, ::5] = 0.0                           # holes, as in SGM proxies
     proxy[:, 3, 4] = 200.0                             # >= 192: invalid
+    proxy[1:, :, :24] = 0.0                            # batch: frames with different numbers of holes
     lt = torch.as_tensor(left).cuda(); rt = torch.as_tensor(right).cuda()
     net = Nets.get_stereo_net('MADNet', dict(left_img=lt, right_img=rt, split_layers=[None], sequence=True, train_portion='BEGIN',
                                              bulkhead=(mode == 'MAD'), warping=True, context_net=True, radius_d=2, stride=1))
@@ -232,12 +246,12 @@ def test_mad_golden_gradients():
                 assert np.abs(got - g[key]).max() < TOL_GRAD * max(np.abs(g[key]).max(), 1e-3 * ref_norm), key
 
 
-@pytest.mark.parametrize('hw', [(64, 128), (100, 200)])
+@pytest.mark.parametrize('hw', [(64, 128), (100, 200), B3])
 def test_full_step_parity(hw):
     from madstereo.synthetic import make_pair
     from oracle.adaptation import OracleAdapter
-    h, w = hw
-    left, right, _ = make_pair(h, w, seed=3)
+    h, w, batch = hwb(hw)
+    left, right, _ = make_pair(h, w, seed=3, batch=batch)
     net, ad, params, lt, rt = build(left, right, 'FULL')
     orc = OracleAdapter(params, mode='FULL', lr=1e-4)
     prev = params
@@ -317,16 +331,27 @@ def test_sequential_sampler_and_reward_bookkeeping():
 def test_prefetch_pipeline_matches_serial_input_path():
     """step(prefetch=next) stages the next frame's host buffers on a side stream while the current frame computes;
     the sequence of losses and the adapted weights must be identical to the serial path (same kernels, same order)."""
+    _check_prefetch_pipeline(np.float32)
+
+
+def test_prefetch_pipeline_matches_serial_input_path_uint8():
+    """The same with uint8 frames: the staging buffers are uint8 and the conversion runs after the device copy."""
+    _check_prefetch_pipeline(np.uint8)
+
+
+def _check_prefetch_pipeline(dtype):
     from madstereo.synthetic import make_pair
     import Nets
     from madstereo.adaptation import OnlineAdaptation
     from oracle.madnet import init_params
     frames = [make_pair(64, 128, seed=10 + i)[:2] for i in range(3)]
+    if dtype == np.uint8:
+        frames = [(np.round(l).astype(np.uint8), np.round(r).astype(np.uint8)) for l, r in frames]
     host = [(torch.from_numpy(l).pin_memory(), torch.from_numpy(r).pin_memory()) for l, r in frames]
     cfg = json.load(open(os.path.join(PKG, 'block_config', 'MadNet_full.json')))
 
     def run(pipelined):
-        net = Nets.get_stereo_net('MADNet', dict(left_img=host[0][0].cuda(), right_img=host[0][1].cuda(), split_layers=[None],
+        net = Nets.get_stereo_net('MADNet', dict(left_img=host[0][0].float().cuda(), right_img=host[0][1].float().cuda(), split_layers=[None],
                                                  sequence=True, train_portion='BEGIN', bulkhead=True))
         ad = OnlineAdaptation(net, mode='MAD', train_config=cfg, sample_mode='SEQUENTIAL')
         ad.load_weights(init_params(seed=42))

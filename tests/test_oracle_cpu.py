@@ -221,3 +221,24 @@ def test_oracle_matches_reference_graph_at_padded_size():
     for k in range(5):
         out = OracleAdapter(params, mode='MAD', lr=1e-4).step(left, right, k)
         assert abs(out['train_loss'] - float(g['mad%d_loss' % k])) < 2e-6, k
+
+
+def test_oracle_batch_equals_single_frames():
+    """The batch-N reference of the GPU tests (and of N ranks x 1 frame in data-parallel runs): the oracle at batch 3 gives
+    the per-frame disparities of three batch-1 runs, and its loss -- a mean over the batch -- is the mean of theirs.
+    (torch's CPU convolutions choose their blocking by batch size, so fp32 sums are reordered: ~1e-6 relative.)"""
+    from madstereo.synthetic import make_pair
+    from oracle.dispnet import DispNetOracle, init_params as dinit
+    torch.set_num_threads(1)
+    left, right, _ = make_pair(64, 128, seed=3, batch=3)
+    for net in (MadNetOracle(init_params(seed=42)), DispNetOracle(dinit(seed=7))):
+        disps, _ = net.forward(left, right)
+        loss = float(T.reprojection_loss(disps[-1], torch.tensor(left), torch.tensor(right)))
+        losses = []
+        for b in range(3):
+            lb, rb = left[b:b + 1], right[b:b + 1]
+            d1, _ = net.forward(lb, rb)
+            for i, (d, r) in enumerate(zip(disps, d1)):
+                assert d.shape[0] == 3 and _rel(d[b:b + 1].numpy(), r.numpy()) < 1e-5, (type(net).__name__, b, i)
+            losses.append(float(T.reprojection_loss(d1[-1], torch.tensor(lb), torch.tensor(rb))))
+        assert abs(loss - np.mean(losses)) <= 1e-6 * abs(loss), (type(net).__name__, loss, losses)
