@@ -61,8 +61,8 @@ int ms_conv2d_fwd(const float* x, int n, int h, int w, int cin, int x_cs, const 
 int ms_conv2d_dgrad(const float* dy, int n, int oh, int ow, int cout, int dy_cs, const float* weights,
                     float* dx, int h, int w, int cin, int dx_cs, int kh, int kw, int stride, int dilation,
                     float* scratch, void* stream);
-/* Split-16-bit wgmma path (csrc/conv_bf.cu; the engine's default for every eligible layer, MS_CONV_IMPL=fp32 selects
- * the CUDA-core kernels above): operands as two 16-bit planes (x ~= hi + lo), three 16-bit MMAs per K step at the
+/* Split-16-bit wgmma path (csrc/conv_bf.cu; the engine runs every eligible layer on it, the rest on the CUDA-core
+ * kernels above): operands as two 16-bit planes (x ~= hi + lo), three 16-bit MMAs per K step at the
  * bf16/fp16 tensor rate.  Forward operands are fp16 planes of x * act_scale and of w (22 mantissa bits, ~2^-22 relative
  * product error; the power-of-two scale is undone exactly in the epilogue); gradient operands are bf16 planes (16 bits, fp32 exponent
  * range).  GEMM transposed so that M = output channels and N = up to 256 pixels, halo patches by TMA (64-channel K

@@ -395,7 +395,6 @@ void* ms_engine_create(const char* net_name, int B, int H, int W, int radius_d, 
     // images (Nets/MadNet.py:56-66) -> activations up to ~1e4, 1/16 keeps |x| <= 1e6 finite; DispNet normalises its input
     // to [-0.4, 0.6] (Nets/DispNet.py:59-73) -> activations O(1e-3 .. 10), 64 lifts them out of fp16's subnormal range
     e->act_scale = e->net == 1 ? 64.f : 0.0625f;
-    if (const char* as = getenv("MS_ACT_SCALE")) { const float v = (float)atof(as); if (v > 0.f) e->act_scale = v; }
     e->finalize_groups(nullptr, 0);
     return e;
 }

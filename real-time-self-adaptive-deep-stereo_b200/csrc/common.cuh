@@ -44,7 +44,7 @@ void add_launches(long long n);
 
 // ---------------------------------------------------------------------------------------------
 // programmatic dependent launch (PDL): every kernel of the step starts with pdl_prologue() and is launched through
-// launch_k(), which sets cudaLaunchAttributeProgrammaticStreamSerialization (MS_PDL=0 disables).  A kernel's CTAs may
+// launch_k(), which sets cudaLaunchAttributeProgrammaticStreamSerialization.  A kernel's CTAs may
 // then become resident while the previous kernel of the stream is still draining; nothing of the kernel body runs before
 // that kernel has completed and flushed (griddepcontrol.wait), so the data dependences of the stream order are intact --
 // what overlaps is launch latency and, in the tensor-core kernels, barrier set-up.  Inside the captured step graph the
@@ -56,9 +56,6 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_prologue() { pdl_trigger(); pdl_wait(); }
 #endif
 bool pdl_enabled();
-// MS_CARVEOUT=1: every kernel launched through launch_k() asks for the maximum shared-memory carve-out, so consecutive
-// kernels of the step never make an SM re-partition L1 / shared memory (experiment; off by default)
-void carveout_once(const void* kernel);
 void pdl_set_suppressed(bool s);      // the instrumented (event-node) graphs of ms_engine_profile(2) are captured without PDL edges
 template <typename... KArgs, typename... Args>
 inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
@@ -68,7 +65,6 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    carveout_once(reinterpret_cast<const void*>(kernel));
     (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);      // errors surface in check_launch()
 }
 

@@ -581,35 +581,20 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
     //      how many of the SMs work in the last wave: cost = waves x (N + fixed overhead in pixel units); ties go to the
     //      taller tile (smaller halo).
     const int mblocks = Mpad / 128;
-    static int force_n = -1, tile_search = -1;
-    if (force_n < 0) { const char* e = getenv("MS_BF_N"); force_n = e ? atoi(e) : 0; }
-    if (tile_search < 0) { const char* e = getenv("MS_BF_TILE_SEARCH"); tile_search = (e && e[0] == '0') ? 0 : 1; }
     int N = 64, TW = 8;
-    if (force_n || !tile_search) {
-        const int cand_n[2] = {128, 64};
-        for (int ci = 0; ci < 2; ++ci) {
-            const int n = cand_n[ci];
-            const int tw = 8;
-            const int th = n / tw;
+    long best = -1; int best_th = 0;
+    const int tws[3] = {8, 16, 32};
+    for (int wi = 0; wi < 3; ++wi) {
+        const int tw = tws[wi];
+        if (tw * sx > 256) continue;
+        for (int th = 1; th * tw <= BF_MAX_N; ++th) {
+            const int n = th * tw;
+            if (n < 64 || (n & 31)) continue;
+            if ((th + max_off) * sx > 256) continue;
             const long tiles = (long)g.y.n * cdiv(Wj, tw) * cdiv(Hj, th) * mblocks;
-            const bool take = force_n ? (n == force_n || ci == 1) : (tiles >= 100 || ci == 1);
-            if (take) { N = n; TW = tw; break; }
-        }
-    } else {
-        long best = -1; int best_th = 0;
-        const int tws[3] = {8, 16, 32};
-        for (int wi = 0; wi < 3; ++wi) {
-            const int tw = tws[wi];
-            if (tw * sx > 256) continue;
-            for (int th = 1; th * tw <= BF_MAX_N; ++th) {
-                const int n = th * tw;
-                if (n < 64 || (n & 31)) continue;
-                if ((th + max_off) * sx > 256) continue;
-                const long tiles = (long)g.y.n * cdiv(Wj, tw) * cdiv(Hj, th) * mblocks;
-                // (halo rows are loaded, not multiplied: a quarter weight keeps 32 x 2 tiles for the cases that save a wave)
-                const long cost = cdiv((int)std::min<long>(tiles, 1 << 30), NUM_SMS) * (long)(n + 32 + max_off * tw / 4);
-                if (best < 0 || cost < best || (cost == best && th > best_th)) { best = cost; best_th = th; N = n; TW = tw; }
-            }
+            // (halo rows are loaded, not multiplied: a quarter weight keeps 32 x 2 tiles for the cases that save a wave)
+            const long cost = cdiv((int)std::min<long>(tiles, 1 << 30), NUM_SMS) * (long)(n + 32 + max_off * tw / 4);
+            if (best < 0 || cost < best || (cost == best && th > best_th)) { best = cost; best_th = th; N = n; TW = tw; }
         }
     }
     const int TH = N / TW;
@@ -634,17 +619,11 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
     const size_t pslot = 2 * (size_t)p.slot_bytes;
     const size_t budget = 220 * 1024;
     MS_REQUIRE(2 * pslot + 2 * wslot <= budget, "conv_bf: patch does not fit shared memory");
-    // MS_BF_SMEM_KB: cap on the two rings (default: all of the SM).  A CTA that leaves half of the shared memory free lets the
-    // NEXT kernel's CTA become resident while this one drains (programmatic dependent launch: barrier set-up and
-    // tensor-map fetch then overlap); deeper rings only help while loads are the bound.
-    static long ring_cap = -1;
-    if (ring_cap < 0) { const char* e = getenv("MS_BF_SMEM_KB"); ring_cap = e ? std::max(32L, atol(e)) * 1024 : (long)budget; }
-    const size_t grow_budget = std::max<size_t>(std::min<size_t>(budget, (size_t)ring_cap), 2 * pslot + 2 * wslot);
     int NP = 2, NW = 2;
     for (;;) {                                       // grow the two rings alternately while they fit (weights first: smaller)
         bool grew = false;
-        if (NW < 8 && (size_t)NP * pslot + (size_t)(NW + 1) * wslot <= grow_budget && NW <= 2 * NP) { ++NW; grew = true; }
-        if (NP < 4 && (size_t)(NP + 1) * pslot + (size_t)NW * wslot <= grow_budget) { ++NP; grew = true; }
+        if (NW < 8 && (size_t)NP * pslot + (size_t)(NW + 1) * wslot <= budget && NW <= 2 * NP) { ++NW; grew = true; }
+        if (NP < 4 && (size_t)(NP + 1) * pslot + (size_t)NW * wslot <= budget) { ++NP; grew = true; }
         if (!grew) break;
     }
     p.NP = NP; p.NW = NW;
@@ -657,21 +636,13 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
     }
     p.wtiles = static_cast<const unsigned char*>(wtiles);
     // ---- split K over (K block, patch) units when the map is too small to fill the GPU (at most 8 ways: the closing
-    //      CTA reads every partial sum)
+    //      CTA reads every partial sum).  The split is as wide as the idle SMs allow: the serial K loop of a grid of a few
+    //      CTAs costs more than the partial-sum round trip.
     const int grid_tiles = p.NB * p.tiles_x * p.tiles_y;
     const int units = p.kblocks * p.n_patches;
     int ksplit = 1;
     if (part && tickets && (long)grid_tiles * mblocks <= NUM_SMS / 2 && units > 1) {
-        static int kmax = -1;
-        if (kmax < 0) { const char* e = getenv("MS_BF_KSPLIT_MAX"); kmax = e ? std::max(1, atoi(e)) : 8; }
-        ksplit = std::min(std::min(units, kmax), std::max(1, NUM_SMS / (grid_tiles * mblocks)));
-        // MS_BF_SPLIT_CYCLES = c: split only while a CTA's share of the main loop stays above c MMA cycles (taps x k16 x
-        // 3 products x N/2).  The default keeps every split (c = 1): the serial K loop of a grid of a few CTAs costs more
-        // than the partial-sum round trip.
-        static int min_cyc = -1;
-        if (min_cyc < 0) { const char* e = getenv("MS_BF_SPLIT_CYCLES"); min_cyc = e ? atoi(e) : 1; }
-        const long loop_cycles = (long)p.kblocks * nt * (p.kch / 16) * 3 * (N / 2);
-        ksplit = (int)std::max<long>(1, std::min<long>(ksplit, loop_cycles / std::max(min_cyc, 1)));
+        ksplit = std::min(std::min(units, 8), std::max(1, NUM_SMS / (grid_tiles * mblocks)));
         while (ksplit > 1 && (size_t)ksplit * grid_tiles * mblocks * N * 128 > conv_bf_part_floats()) --ksplit;
         if ((size_t)grid_tiles * mblocks > conv_bf_ticket_words()) ksplit = 1;
     }

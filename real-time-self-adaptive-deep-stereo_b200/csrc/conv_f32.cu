@@ -251,11 +251,7 @@ size_t conv_gemm_part_floats() { return (size_t)8 << 20; }      // 32 MB split-K
 int conv_gemm(const ConvGemm& p_in, cudaStream_t st) {
     ConvGemm p = p_in;
     MS_REQUIRE(p.x.n == p.y.n, "conv_gemm: batch mismatch");
-    {
-        static int small_env = -1;
-        if (small_env < 0) { const char* e = getenv("MS_CONV_SMALL"); small_env = (e && e[0] == '0') ? 0 : 1; }
-        if (small_env && conv_small_fwd_supported(p)) return conv_small_fwd(p, st);     // cin = 3 (conv_small.cu)
-    }
+    if (conv_small_fwd_supported(p)) return conv_small_fwd(p, st);     // cin = 3 (conv_small.cu)
     const size_t Mz = (size_t)p.y.n * p.y.h * p.y.w;
     MS_REQUIRE(Mz < (1u << 30), "conv_gemm: too many output pixels");
     const int M = (int)Mz;
@@ -495,18 +491,13 @@ int conv_wgrad(const ConvWgrad& p, cudaStream_t st) {
     MS_REQUIRE(Pz < (1u << 30), "conv_wgrad: too many pixels");
     const int P = (int)Pz;
     const int taps = p.kh * p.kw, ci = p.x.c, co = p.dy.c;
-    {   // single output channel (disparity heads): dedicated reduction kernel, conv_head.cu
-        static int heads = -1;
-        if (heads < 0) { const char* e = getenv("MS_HEADS"); heads = (e && e[0] == '0') ? 0 : 1; }
-        if (heads && conv_head_wgrad_supported(p) && p.workspace_floats >= conv_head_wgrad_workspace_floats(p)) return conv_head_wgrad(p, st);
-    }
+    // single output channel (disparity heads): dedicated reduction kernel, conv_head.cu
+    if (conv_head_wgrad_supported(p) && p.workspace_floats >= conv_head_wgrad_workspace_floats(p)) return conv_head_wgrad(p, st);
     int tm, tn; wgrad_tiles(ci, co, tm, tn);
     const int mtiles = cdiv(ci, 16 * tm), ntiles = cdiv(co, 16 * tn);
     const size_t wn = (size_t)taps * ci * co;
     const int nb = bias_blocks(Pz);
-    static int small_env = -1;
-    if (small_env < 0) { const char* e = getenv("MS_CONV_SMALL"); small_env = (e && e[0] == '0') ? 0 : 1; }
-    const bool small = small_env && conv_small_wgrad_supported(p) &&
+    const bool small = conv_small_wgrad_supported(p) &&
                        p.workspace_floats >= conv_small_wgrad_workspace_floats(taps, ci, co, Pz) + (size_t)nb * co;
     int split = wgrad_split(taps * mtiles * ntiles, Pz);
     int chunk = cdiv(P, split);

@@ -6,9 +6,9 @@
 // On these layers the generic gather GEMM is far from the HBM bound for conv1 forward (0.2 GFLOP, 27 MB) and for the
 // conv1 / conv2 weight gradients (432 / 2304 outputs reduced over 245 760 pixels: a 16 x 16 output tile leaves the GEMM
 // kernel with 9 CTAs per K split).
-//   forward  : one thread computes two adjacent output pixels x all output channels; the weights sit in shared memory
-//              and are read as broadcast float4.  (16 -> 16 | 32 instantiations exist but are
-//              opt-in: without a staged input patch they are slower than the gather GEMM, see conv_small_fwd_supported.)
+//   forward  : 3 -> 16: one thread computes two adjacent output pixels x all output channels; the weights sit in shared
+//              memory and are read as broadcast float4.  16 -> 16: the same arithmetic on an input patch staged in
+//              shared memory (conv_c16_tiled_kernel).
 //   wgrad    : a thread owns one input channel ("role") and keeps all 9 taps x 16 output channels = 144 partial sums
 //              in registers while it walks its share of the pixels (9 input loads + 16 dY loads per 144 FMAs, next
 //              pixel prefetched); lanes of equal role are combined by shuffles, warps through shared memory, CTAs by
@@ -23,7 +23,7 @@ namespace ms {
 static __host__ __device__ bool al16s(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // ---------------------------------------------------------------------------------------------
-// forward / stride-1 dgrad gather, 3x3, (cin, cout) in {(3,16), (16,16), (16,32)}
+// forward gather, 3x3, 3 -> 16
 // ---------------------------------------------------------------------------------------------
 constexpr int CS_NT = 128;
 
@@ -56,16 +56,8 @@ __global__ void __launch_bounds__(CS_NT) conv_small_fwd_kernel(ConvGemm p, int p
             const int ix = (ox0 + pi) * p.mul + p.off_x + tx * p.step;
             const bool ok = rok && ix >= 0 && ix < p.x.w;
             const float* s = ximg + ((size_t)(ok ? iy : 0) * p.x.w + (ok ? ix : 0)) * p.x.cs;
-            if constexpr (CIN % 4 == 0) {
 #pragma unroll
-                for (int c4 = 0; c4 < CIN / 4; ++c4) {
-                    const float4 v = ok ? __ldg(reinterpret_cast<const float4*>(s) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    xin[pi][4 * c4] = v.x; xin[pi][4 * c4 + 1] = v.y; xin[pi][4 * c4 + 2] = v.z; xin[pi][4 * c4 + 3] = v.w;
-                }
-            } else {
-#pragma unroll
-                for (int c = 0; c < CIN; ++c) xin[pi][c] = ok ? __ldg(s + c) : 0.f;
-            }
+            for (int c = 0; c < CIN; ++c) xin[pi][c] = ok ? __ldg(s + c) : 0.f;
         }
         const float4* wt = reinterpret_cast<const float4*>(ws + tap * CIN * CO);
 #pragma unroll
@@ -111,8 +103,7 @@ __global__ void __launch_bounds__(CS_NT) conv_small_fwd_kernel(ConvGemm p, int p
 // 16 -> 16, 3x3, stride 1 (conv2 forward and its dgrad): shared-memory staged version.  A CTA owns an 8 x 32 output tile;
 // the 10 x 34 input patch is loaded with coalesced 128-bit loads into shared memory with a 20-float pixel pitch (a
 // quarter-warp's 128-bit reads at one-pixel lane stride then hit 32 distinct banks); a thread computes pixels (r, c) and
-// (r, c + 16) so that lanes stay one pixel apart.  Default (MS_CONV_SMALL16=2; 0 = gather GEMM, 1 = untiled direct
-// kernels): validated with the ops + MADNet GPU suites.
+// (r, c + 16) so that lanes stay one pixel apart.
 // ---------------------------------------------------------------------------------------------
 constexpr int T16_TH = 8, T16_TW = 32, T16_PH = T16_TH + 2, T16_PW = T16_TW + 2, T16_PS = 20, T16_NT = 128;
 
@@ -201,12 +192,6 @@ __global__ void __launch_bounds__(T16_NT) conv_c16_tiled_kernel(ConvGemm p, int 
     }
 }
 
-static int small16_mode() {
-    static int m = -1;
-    if (m < 0) { const char* e = getenv("MS_CONV_SMALL16"); m = e ? atoi(e) : 2; }
-    return m;
-}
-
 static bool conv_c16_tiled_supported(const ConvGemm& p) {
     return p.x.c == 16 && p.y.c == 16 && p.kh == 3 && p.kw == 3 && p.div == 1 && p.mul == 1 && (p.step == 1 || p.step == -1) &&
            p.x.h == p.y.h && p.x.w == p.y.w && p.x.n == p.y.n && (p.x.cs & 3) == 0 && al16s(p.x.p) && al16s(p.wmat) &&
@@ -216,17 +201,13 @@ static bool conv_c16_tiled_supported(const ConvGemm& p) {
 bool conv_small_fwd_supported(const ConvGemm& p) {
     if (p.kh != 3 || p.kw != 3 || p.div != 1 || p.mul < 1 || p.x.n != p.y.n || p.alpha > 1.f || p.alpha < 0.f) return false;
     if (p.x.c == 3 && p.y.c == 16) return true;
-    // The untiled 16-channel instantiations are opt-in (MS_CONV_SMALL16=1): slower than the gather GEMM -- one thread
-    // reading its pixels' 64-byte channel rows straight from global memory is LSU-bound (32 cache lines per load
-    // instruction).  The default (=2) is the shared-memory
-    // tiled 16->16 stride-1 kernel above.
-    if (small16_mode() == 2 && conv_c16_tiled_supported(p)) return true;
-    if (small16_mode() == 1 && p.x.c == 16 && (p.y.c == 16 || p.y.c == 32)) return (p.x.cs & 3) == 0 && al16s(p.x.p);
-    return false;
+    // 16 channels only with the input patch staged in shared memory: one thread reading its pixels' 64-byte channel
+    // rows straight from global memory is LSU-bound (32 cache lines per load instruction), slower than the gather GEMM
+    return conv_c16_tiled_supported(p);
 }
 
 int conv_small_fwd(const ConvGemm& p, cudaStream_t st) {
-    if (small16_mode() == 2 && conv_c16_tiled_supported(p)) {
+    if (conv_c16_tiled_supported(p)) {
         const int tiles_x = cdiv(p.y.w, T16_TW), tiles_y = cdiv(p.y.h, T16_TH);
         launch_k(conv_c16_tiled_kernel, dim3((unsigned)(tiles_x * tiles_y * p.y.n)), dim3(T16_NT), 0, st, p, tiles_x, tiles_y);
         return check_launch("conv_c16_tiled");
@@ -235,9 +216,7 @@ int conv_small_fwd(const ConvGemm& p, cudaStream_t st) {
     const size_t total = (size_t)p.y.n * p.y.h * pairs_per_row;
     MS_REQUIRE(total < (1u << 30), "conv_small_fwd: too many output pixels");
     const unsigned grid = (unsigned)cdivz(total, CS_NT);
-    if (p.x.c == 3) launch_k(conv_small_fwd_kernel<3, 16>, dim3(grid), dim3(CS_NT), 0, st, p, pairs_per_row, (int)total);
-    else if (p.y.c == 16) launch_k(conv_small_fwd_kernel<16, 16>, dim3(grid), dim3(CS_NT), 0, st, p, pairs_per_row, (int)total);
-    else launch_k(conv_small_fwd_kernel<16, 32>, dim3(grid), dim3(CS_NT), 0, st, p, pairs_per_row, (int)total);
+    launch_k(conv_small_fwd_kernel<3, 16>, dim3(grid), dim3(CS_NT), 0, st, p, pairs_per_row, (int)total);
     return check_launch("conv_small_fwd");
 }
 

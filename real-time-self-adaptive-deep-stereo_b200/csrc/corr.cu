@@ -294,7 +294,7 @@ __global__ void __launch_bounds__(CORR_NT) corr_fwd2_kernel(CorrFwd p, int TW, i
 // and each lane owns CPL >= 3 consecutive chunks; the left chunk is held in registers across the nd displacements;
 // shared-memory tiles are stored with an XOR swizzle of the chunk index (low 3 bits ^ column&7) so that lane=column
 // accesses are bank-conflict free.  Tiles are staged with coalesced 128-bit loads (the swizzle rules out the 1-D bulk
-// copy used by v1/v2, which remain available: MS_CORR_V=1|2).
+// copy used by v1/v2, which serve the shapes v3 declines).
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ int swz_m(int q, int col, int m) { return (q & ~m) | ((q ^ col) & m); }
 
@@ -431,11 +431,6 @@ __global__ void __launch_bounds__(CORR_NT) corr_fwd3_kernel(CorrFwd p, int TW, i
     }
 }
 
-static bool corr_use_tma() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("MS_CORR_NO_TMA"); v = (e && e[0] == '1') ? 0 : 1; }
-    return v == 1;
-}
 int corr_init();
 static bool a16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
@@ -459,16 +454,14 @@ int corr_fwd(const CorrFwd& p, cudaStream_t st) {
     MS_REQUIRE(p.stride >= 1, "corr_fwd: stride");
     const bool warped = p.u != nullptr;
     const int nd = (2 * p.max_disp) / p.stride + 1;
-    int tma = corr_use_tma() && p.lcs == p.C && p.rcs == p.C;
+    int tma = p.lcs == p.C && p.rcs == p.C;
     if (corr_init()) return -1;
-    static int ver = -1;
-    if (ver < 0) { const char* e = getenv("MS_CORR_V"); ver = e ? atoi(e) : 4; }
-    if (ver >= 4 && corr_mma_supported(p)) return corr_mma(p, st);      // DispNet: 81 displacements as a banded tensor-core product
-    if (ver >= 4) {                                     // MADNet cost volume (d=2, C%32==0): tensor-map TMA kernel, corr_tma.cu
+    if (corr_mma_supported(p)) return corr_mma(p, st);      // DispNet: 81 displacements as a banded tensor-core product
+    {                                                   // MADNet cost volume (d=2, C%32==0): tensor-map TMA kernel, corr_tma.cu
         const int r = corr_fwd4(p, st);
         if (r <= 0) return r;
     }
-    if (ver >= 3) {
+    {
         const int nchunk = p.C / 4;
         const int LP = nchunk >= 24 ? 8 : (nchunk >= 16 ? 4 : (nchunk >= 8 ? 2 : 1));
         // v3 for C<=32 (level 2, which moves most of the bytes), v2 for wider features / nd=81
@@ -486,12 +479,10 @@ int corr_fwd(const CorrFwd& p, cudaStream_t st) {
             }
         }
     }
-    if (ver >= 2) {
+    {
         // tile width: aim at >= 3 CTAs per SM
-        static int tw_env = -1, slack_env = -1;
-        if (tw_env < 0) { const char* e = getenv("MS_CORR_TW"); tw_env = e ? atoi(e) : 0; const char* f = getenv("MS_CORR_SLACK"); slack_env = f ? atoi(f) : 0; }
-        int TW = std::min(p.w, tw_env > 0 ? tw_env : (p.C >= 128 ? 32 : 64));
-        const int RCAP = warped ? TW + 2 * p.max_disp + (slack_env > 0 ? slack_env : 64) : 0;
+        const int TW = std::min(p.w, p.C >= 128 ? 32 : 64);
+        const int RCAP = warped ? TW + 2 * p.max_disp + 64 : 0;
         const size_t smem = ((size_t)TW + (size_t)(TW + 2 * p.max_disp) + (size_t)RCAP) * p.C * 4 +
                             (size_t)(TW + 2 * p.max_disp) * sizeof(Tap) + 64;
         if (smem <= 200 * 1024) {
@@ -668,11 +659,7 @@ int corr_bwd(const CorrBwd& p, cudaStream_t st) {
                "corr_bwd: C and strides must be multiples of 4");
     MS_REQUIRE(a16(p.left) && a16(p.right) && a16(p.dleft) && a16(p.dright), "corr_bwd: pointers must be 16B aligned");
     MS_REQUIRE(!p.add_left_slice || (p.dcs % 4 == 0 && a16(p.dcost)), "corr_bwd: dcost slice alignment");
-    {
-        static int ver = -1;
-        if (ver < 0) { const char* e = getenv("MS_CORR_V"); ver = e ? atoi(e) : 4; }
-        if (ver >= 4 && corr_mma_bwd_supported(p)) return corr_mma_bwd(p, st);     // DispNet: banded tensor-core products
-    }
+    if (corr_mma_bwd_supported(p)) return corr_mma_bwd(p, st);     // DispNet: banded tensor-core products
     const bool warped = p.u != nullptr;
     const int nd = (2 * p.max_disp) / p.stride + 1;
     const size_t budget = 220 * 1024;
@@ -694,7 +681,7 @@ int corr_bwd(const CorrBwd& p, cudaStream_t st) {
     }
     const size_t WIN = warped ? p.w : TW + 2 * p.max_disp;
     size_t smem = 2 * WIN * p.C * 4 + (warped ? (size_t)TW * p.C * 4 : 0) + WIN * nd * 4 + (warped ? (size_t)p.w * 4 : 0) + 64;
-    int tma = corr_use_tma() && p.lcs == p.C && p.rcs == p.C;
+    int tma = p.lcs == p.C && p.rcs == p.C;
     if (corr_init()) return -1;
     dim3 grid(cdiv(p.w, TW), p.B * p.h);
     launch_k(corr_bwd_kernel, dim3(grid), dim3(CORR_NT), smem, st, p, TW, nd, tma);

@@ -1,4 +1,4 @@
-// Correlation forward v4: tensor-map TMA staging, one (or two) threads per pixel.
+// Correlation forward v4: tensor-map TMA staging, two threads per pixel.
 //
 // Same operator as corr.cu (reference Nets/sharedLayers.py:23-51 correlation, Nets/MadNet.py:370-375 concat,
 // Nets/MadNet.py:400-436 linear warp; native launcher Nets/Native/shift_corr.cu.cc:193-233), specialised for the MADNet
@@ -14,13 +14,12 @@
 //   * out-of-image columns are zero rows (TMA zero fill for the un-warped window, zero taps for the warped one), so the
 //     displacement loop has no bounds predicates;
 //   * the warped right row RW is materialised once per tile in shared memory, every RW column feeds 5 outputs;
-//   * each pixel is owned by LP (1 or 2) lanes that keep the 5 running sums in registers; results leave as two 128-bit
+//   * each pixel is owned by LP = 2 lanes that keep the 5 running sums in registers; results leave as two 128-bit
 //     stores per pixel into the concat buffer ([c0 c1 c2 c3][c4 u 0 0]).
 // The right window of a warped tile is data dependent: taps are computed first, the window [min tap, max tap] is then
 // fetched by one TMA copy per 32-channel block (bounded by RB rows; taps outside read global memory directly).
 #include <algorithm>
 #include <climits>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "corr_common.cuh"
@@ -51,20 +50,20 @@ __device__ __forceinline__ uint32_t rowkey(uint32_t tile_s, int r) { return (til
 struct Corr4Params {
     CorrFwd p;
     int TW, WB, RB, ncb;     // tile width, RW rows (>= TW+4), raw right window rows, 32-channel blocks
-    int store_o, store_o2;   // left -> concat copy by TMA store
+    int store_o2;            // left -> context buffer copy by TMA store (the concat buffer's copy always is)
     float invC;
 };
 
 // float4 index of chunk q of row r in 32-channel block cb of a [ncb][rows][8] swizzled tile
 __device__ __forceinline__ int t4(int cb, int rows, int r, int q) { return ((cb * rows + r) << 3) + (q ^ (r & 7)); }
 
-template <int LP, int NCB_CT>     // NCB_CT > 0: number of 32-channel blocks known at compile time (loops unroll)
+template <int NCB_CT>     // NCB_CT > 0: number of 32-channel blocks known at compile time (loops unroll)
 __global__ void __launch_bounds__(256) corr_fwd4_kernel(const __grid_constant__ CUtensorMap mapL,
                                                         const __grid_constant__ CUtensorMap mapR,
                                                         const __grid_constant__ CUtensorMap mapO,
                                                         const __grid_constant__ CUtensorMap mapO2, const Corr4Params k) {
     pdl_prologue();
-    constexpr int ND = 5, D = 2, QPL = 8 / LP;
+    constexpr int ND = 5, D = 2, LP = 2, QPL = 8 / LP;
     const CorrFwd& p = k.p;
     extern __shared__ unsigned char smem_dyn[];
     __shared__ __align__(8) uint64_t barL, barR;
@@ -128,25 +127,23 @@ __global__ void __launch_bounds__(256) corr_fwd4_kernel(const __grid_constant__ 
         }
     }
     // ---- left tile -> concat buffer(s)
-    const bool any_store = p.copy_left && (k.store_o || (p.out2 && k.store_o2));
-    if (tid == 0 && any_store) {
+    if (tid == 0 && p.copy_left) {
         mb_wait(&barL, 0);
         for (int cb = 0; cb < ncb; ++cb) {
-            if (k.store_o) tma_store_3d(&mapO, Ls + (size_t)cb * TW * 8, cb * 32, x0, row);
+            tma_store_3d(&mapO, Ls + (size_t)cb * TW * 8, cb * 32, x0, row);
             if (p.out2 && k.store_o2) tma_store_3d(&mapO2, Ls + (size_t)cb * TW * 8, cb * 32, x0, row);
         }
         bulk_commit();
     }
     mb_wait(&barL, 0);
-    if (p.copy_left && (!k.store_o || (p.out2 && !k.store_o2))) {
-        float* o2row = p.out2 ? p.out2 + (size_t)row * w * p.o2cs : nullptr;
+    if (p.copy_left && p.out2 && !k.store_o2) {
+        float* o2row = p.out2 + (size_t)row * w * p.o2cs;
         const int per = ncb * 8;
         for (int e = tid; e < TW * per; e += nthr) {
             const int j = e / per, r = e - j * per, cb = r >> 3, q = r & 7;
             if (x0 + j >= w) continue;
             const float4 v = Ls[t4(cb, TW, j, q)];
-            if (!k.store_o) *reinterpret_cast<float4*>(orow + (size_t)(x0 + j) * p.ocs + cb * 32 + q * 4) = v;
-            if (o2row && !k.store_o2) *reinterpret_cast<float4*>(o2row + (size_t)(x0 + j) * p.o2cs + cb * 32 + q * 4) = v;
+            *reinterpret_cast<float4*>(o2row + (size_t)(x0 + j) * p.o2cs + cb * 32 + q * 4) = v;
         }
     }
     const int sub = tid % LP, pl = tid / LP, npl = nthr / LP;          // lane within pixel, pixel slot
@@ -248,10 +245,9 @@ __global__ void __launch_bounds__(256) corr_fwd4_kernel(const __grid_constant__ 
             }
         }
     }
-    if (tid == 0 && any_store) bulk_wait_read0();       // the TMA stores read Ls: keep the CTA's smem alive until done
+    if (tid == 0 && p.copy_left) bulk_wait_read0();       // the TMA stores read Ls: keep the CTA's smem alive until done
 }
 
-static int env_int(const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; }
 static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // 3-D view {channels, w, B*h} of an NHWC tensor with channel stride cs; box {32, rows, 1}
@@ -271,50 +267,41 @@ int corr_fwd4(const CorrFwd& p, cudaStream_t st) {
     if (p.stride != 1 || p.max_disp != 2 || p.C % 32 != 0 || p.C > 256 || p.w < 8) return 1;
     if ((p.lcs & 3) || (p.rcs & 3) || !al16(p.left) || !al16(p.right) || !al16(p.out)) return 1;
     if (p.copy_left && (p.ocs & 3)) return 1;
-    static int tw_env = -2, lp_env, st_env, slack_env;
-    if (tw_env == -2) {
-        lp_env = env_int("MS_CORR4_LP", 2); st_env = env_int("MS_CORR4_ST", 1); slack_env = env_int("MS_CORR4_SLACK", 16);
-        tw_env = env_int("MS_CORR4_TW", 0);
-    }
-    const int LP = lp_env == 1 ? 1 : 2;
     const int ncb = p.C / 32;
-    // 64-pixel tiles (7 CTAs per SM at C=32) rather than 128; slack 16 rather than 32
-    int TW = tw_env > 0 ? tw_env : std::max(32, std::min(64, (128 / ncb + 7) / 8 * 8));
-    TW = std::min(TW, 256 / LP);
+    // 64-pixel tiles (7 CTAs per SM at C=32) rather than 128; slack 16 rather than 32.  Two lanes per pixel: at most
+    // 128 threads
+    int TW = std::max(32, std::min(64, (128 / ncb + 7) / 8 * 8));
     TW = std::min(TW, (p.w + 7) / 8 * 8);
     TW = std::max(8, TW / 8 * 8);
     const int WB = (TW + 4 + 7) / 8 * 8;
-    const int RB = warped ? std::min(256, (TW + 4 + std::max(8, slack_env) + 7) / 8 * 8) : 0;
+    const int RB = warped ? std::min(256, (TW + 4 + 16 + 7) / 8 * 8) : 0;
     const size_t smem = (size_t)ncb * (TW + WB + RB) * 128 + (size_t)WB * sizeof(Tap) + 1024 + 64;
     if (smem > 200 * 1024) return 1;
 
     Corr4Params k;
     k.invC = 1.f / (float)p.C;
     k.p = p; k.TW = TW; k.WB = WB; k.RB = RB; k.ncb = ncb;
-    k.store_o = (p.copy_left && st_env) ? 1 : 0;
-    k.store_o2 = (p.copy_left && p.out2 && st_env && (p.o2cs & 3) == 0 && al16(p.out2)) ? 1 : 0;
+    k.store_o2 = (p.copy_left && p.out2 && (p.o2cs & 3) == 0 && al16(p.out2)) ? 1 : 0;
     const int rows = p.B * p.h;
     CUtensorMap mL, mR, mO, mO2;
     if (feat_map(&mL, p.left, p.C, p.lcs, p.w, rows, TW)) return -1;
     if (feat_map(&mR, p.right, p.C, p.rcs, p.w, rows, warped ? RB : WB)) return -1;
     mO = mL; mO2 = mL;
-    if (k.store_o && feat_map(&mO, p.out, p.C, p.ocs, p.w, rows, TW)) return -1;
+    if (p.copy_left && feat_map(&mO, p.out, p.C, p.ocs, p.w, rows, TW)) return -1;
     if (k.store_o2 && feat_map(&mO2, p.out2, p.C, p.o2cs, p.w, rows, TW)) return -1;
 
     static bool attr = false;
     if (!attr) {
-        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
-        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<2, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
-        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
-        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<2, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
+        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
+        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
+        MS_CHECK_CUDA(cudaFuncSetAttribute(corr_fwd4_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
         attr = true;
     }
     const dim3 grid(cdiv(p.w, TW), rows);
-    const int threads = (TW * LP + 31) / 32 * 32;
-    if (LP == 1) launch_k(corr_fwd4_kernel<1, 0>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
-    else if (ncb == 1) launch_k(corr_fwd4_kernel<2, 1>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
-    else if (ncb == 2) launch_k(corr_fwd4_kernel<2, 2>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
-    else launch_k(corr_fwd4_kernel<2, 0>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
+    const int threads = (TW * 2 + 31) / 32 * 32;
+    if (ncb == 1) launch_k(corr_fwd4_kernel<1>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
+    else if (ncb == 2) launch_k(corr_fwd4_kernel<2>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
+    else launch_k(corr_fwd4_kernel<0>, dim3(grid), dim3(threads), smem, st, mL, mR, mO, mO2, k);
     return check_launch("corr_fwd4");
 }
 

@@ -41,12 +41,6 @@ Engine::Engine()
     gemm_part = nullptr; weights_dirty = true;
     gstream = nullptr; ev_in = nullptr; ev_out = nullptr;
     wstream = nullptr; ev_fork = nullptr; ev_join = nullptr; wstream_dirty = false;
-    { const char* e8 = getenv("MS_WGRAD_OVERLAP"); use_overlap = (e8 && e8[0] == '0') ? 0 : 1; }
-    { const char* e2 = getenv("MS_GRAPHS"); use_graphs = (e2 && e2[0] == '0') ? 0 : 1; }
-    { const char* e4 = getenv("MS_CONV_IMPL"); conv_impl = (e4 && (!strcmp(e4, "fp32") || !strcmp(e4, "0"))) ? 0 : 1; }
-    { const char* e5 = getenv("MS_HEADS"); use_heads = (e5 && e5[0] == '0') ? 0 : 1; }
-    { const char* e7 = getenv("MS_STEM"); use_stem = (e7 && e7[0] == '0') ? 0 : 1; }
-    { const char* e6 = getenv("MS_BF_WGRAD"); use_bf_wgrad = (e6 && e6[0] == '0') ? 0 : 1; }
     wg_xp.hi = wg_xp.lo = nullptr; wg_xp.cs = 0; wg_xp.fmt = 0; wg_xp.scale = 1.f; wg_xp_halfs = 0;
     act_scale = 0.f;
     bf_jobs_dev = nullptr; bf_max_total = 0; bf_part = nullptr; bf_tickets = nullptr;
@@ -54,7 +48,6 @@ Engine::Engine()
 }
 
 void Engine::add_planes(Bump& A, const TView& v, int fmt) {
-    if (conv_impl != 1) return;
     const bool sizing = A.base == nullptr;         // (sizing pass: pointers are null or null + a slice offset -- never dedupe)
     if (!sizing && planes.count(v.p)) return;
     ActPlanes pl;
@@ -217,7 +210,7 @@ size_t Engine::layout(float* base) {
         max_wg = std::max(max_wg, conv_wgrad_workspace_floats(L.kh * L.kw, L.cin, L.cout, pixels));
         max_wt = std::max(max_wt, (size_t)L.kh * L.kw * L.cin * L.cout);
         if (L.cout == 1) max_wg = std::max(max_wg, (size_t)2 * NUM_SMS * ((size_t)L.kh * L.kw * L.cin + 1));    // conv_head_wgrad partials
-        if (conv_impl == 1 && !L.transposed && L.cin >= 3 && L.cout >= 16) {
+        if (!L.transposed && L.cin >= 3 && L.cout >= 16) {
             max_wg = std::max(max_wg, std::min<size_t>(wgrad_bf_workspace_floats(L.kh, L.kw, L.cin, L.cout), (size_t)48 << 20));
             wg_xp_halfs = std::max(wg_xp_halfs, pixels * L.stride * L.stride * (size_t)((L.cin + 7) / 8 * 8));
         }
@@ -294,7 +287,7 @@ size_t Engine::layout(float* base) {
     bfw[1].assign(layers.size(), BfW{nullptr, false});
     bf_jobs.clear(); bf_job_begin.assign(n_groups + 1, 0); bf_job_end.assign(n_groups + 1, 0);
     bf_max_total = 0;
-    for (int gidx = 0; gidx <= n_groups && conv_impl == 1; ++gidx) {
+    for (int gidx = 0; gidx <= n_groups; ++gidx) {
         bf_job_begin[gidx] = (int)bf_jobs.size();
         for (size_t li = 0; li < layers.size(); ++li) {
             const ConvLayer& L = layers[li];
@@ -341,7 +334,7 @@ size_t Engine::layout(float* base) {
         }
         bf_job_end[gidx] = (int)bf_jobs.size();
     }
-    if (conv_impl == 1 && wg_xp_halfs) {
+    if (wg_xp_halfs) {
         wg_xp.hi = alloc((wg_xp_halfs + 1) / 2); wg_xp.lo = alloc((wg_xp_halfs + 1) / 2); wg_xp.fmt = 0;
     }
     bf_part = alloc(conv_bf_part_floats());
@@ -383,22 +376,22 @@ int Engine::conv_fwd(const ConvLayer& L, const TView& x, const TView& y, const f
         p.wmat = wT;
         p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = L.stride;
         const int li_t = (int)(&L - &layers[0]);
-        const bool bf_t = conv_impl == 1 && bfw[0][li_t].ok && conv_bf_supported(p) && planes_of(x);
+        const bool bf_t = bfw[0][li_t].ok && conv_bf_supported(p) && planes_of(x);
         // canonical W is [tap][cout][cin]; the gather GEMM wants [tap][K=cin][N=cout] (the tensor-core path has its own tiles)
         if (!bf_t && transpose_taps(Wt + L.w_off, wT, L.kh * L.kw, L.cout, L.cin, st)) return -1;
     }
     const int li = (int)(&L - &layers[0]);
     prof_begin(CAT_CONV_FWD, st, li);
     int rc;
-    const ActPlanes* xpl = (conv_impl == 1 && bfw[0][li].ok && conv_bf_supported(p)) ? planes_of(x) : nullptr;
-    if (use_heads && conv_head_kind(p) == 1) {
+    const ActPlanes* xpl = (bfw[0][li].ok && conv_bf_supported(p)) ? planes_of(x) : nullptr;
+    if (conv_head_kind(p) == 1) {
         fresh.erase(y.p);
         rc = conv_head(p, st);
-    } else if (use_heads && L.cin == 1 && L.cout == 1 && conv_one_channel_supported(p)) {
+    } else if (L.cin == 1 && L.cout == 1 && conv_one_channel_supported(p)) {
         fresh.erase(y.p);
         p.wmat = Wt + L.w_off;                       // [tap][1][1]: canonical weights serve either orientation
         rc = conv_one_channel(p, st);
-    } else if (use_stem && !L.transposed && (p.wmat = Wt + L.w_off, conv_stem_fwd_supported(p))) {
+    } else if (!L.transposed && (p.wmat = Wt + L.w_off, conv_stem_fwd_supported(p))) {
         // DispNet conv1: 3 real channels per 32-wide K block on the tensor-core path; the CUDA cores do it in a third of the time
         const ActPlanes* ypl = planes_of(y);
         rc = conv_stem_fwd(p, ypl, st);
@@ -439,8 +432,8 @@ int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, cons
         q.workspace = wg_ws; q.workspace_floats = wg_ws_floats; q.accumulate = 0;
         prof_begin(CAT_CONV_WGRAD, st, (int)(&L - &layers[0]));
         int rc = 0;
-        const bool stem_w = use_stem && conv_stem_wgrad_supported(q);
-        const ActPlanes* wxp = (!stem_w && conv_impl == 1 && use_bf_wgrad && wgrad_bf_supported(q)) ? planes_of(x) : nullptr;
+        const bool stem_w = conv_stem_wgrad_supported(q);
+        const ActPlanes* wxp = (!stem_w && wgrad_bf_supported(q)) ? planes_of(x) : nullptr;
         const ActPlanes* wdp = wxp ? planes_of(dpre) : nullptr;
         // the planes of dpre also feed the dgrad below: they are produced on `st` BEFORE the fork
         if (wxp && wdp) rc = ensure_planes(dpre, st);
@@ -455,7 +448,7 @@ int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, cons
             if (!rc) rc = wgrad_bf(q, xb, *wdp, ws);
         } else if (!rc && stem_w) {
             rc = conv_stem_wgrad(q, ws);                 // DispNet conv1
-        } else if (!rc && use_heads && conv_head_wgrad_supported(q)) {
+        } else if (!rc && conv_head_wgrad_supported(q)) {
             rc = conv_head_wgrad(q, ws);                 // single-channel disparity heads
         } else if (!rc) {
             rc = conv_wgrad(q, ws);
@@ -475,8 +468,8 @@ int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, cons
         const int li = (int)(&L - &layers[0]);
         prof_begin(CAT_CONV_DGRAD, st, li);
         int rc;
-        const ActPlanes* xpl = (conv_impl == 1 && bfw[1][li].ok && conv_bf_supported(p)) ? planes_of(dpre) : nullptr;
-        if (use_heads && L.cout == 1 && (p.wmat = Wt + L.w_off, conv_head_kind(p) == 2)) {
+        const ActPlanes* xpl = (bfw[1][li].ok && conv_bf_supported(p)) ? planes_of(dpre) : nullptr;
+        if (L.cout == 1 && (p.wmat = Wt + L.w_off, conv_head_kind(p) == 2)) {
             fresh.erase(dx->p);
             rc = conv_head(p, st);          // [tap][cin][1] == [tap][1][cin]: the canonical weights serve directly
         } else if (xpl) {
@@ -640,7 +633,7 @@ int Engine::loss(int which, int with_grad, int slot, float grad_scale, cudaStrea
 // operands; they share one workspace, so they serialise among themselves while the dgrad chain proceeds on `st`
 int Engine::fork_wgrad(cudaStream_t st, cudaStream_t* ws) {
     *ws = st;
-    if (!use_overlap || profiling || net != 0) return 0;
+    if (profiling || net != 0) return 0;
     if (!wstream) {
         MS_CHECK_CUDA(cudaStreamCreateWithFlags(&wstream, cudaStreamNonBlocking));
         MS_CHECK_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
@@ -848,7 +841,7 @@ int Engine::run_eager(int mode, int group, int disp_mask, int with_update, float
 int Engine::run(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st) {
     MS_REQUIRE(bound, "engine not bound");
     MS_REQUIRE(mode == 0 || mode == 2 || (mode == 1 && group >= 0 && group < n_groups), "run: bad mode/group");
-    if (!use_graphs || profiling == 1) return run_eager(mode, group, disp_mask, with_update, lr, mu, gscale, st);
+    if (profiling == 1) return run_eager(mode, group, disp_mask, with_update, lr, mu, gscale, st);
     if (weights_dirty) {                    // load / restore happened: refresh every tf32 copy outside the graph
         if (prep_layers(-1, st)) return -1;
         weights_dirty = false;

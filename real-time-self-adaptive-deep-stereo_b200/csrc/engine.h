@@ -80,22 +80,17 @@ struct Engine {
     struct Span;
     struct GraphRec { cudaGraphExec_t exec; long long kernels; std::vector<Span>* spans; };
     std::map<GraphKey, GraphRec> graphs;
-    int use_graphs;
     cudaStream_t gstream; cudaEvent_t ev_in, ev_out;   // graphs run on a private stream (the legacy default stream cannot be captured)
     // weight gradients on a side stream: wgrad(layer j) only needs dpre_j and the forward activation, so it runs concurrently
-    // with the dgrad chain (fork / join through events; inside the captured step this becomes a parallel graph branch)
-    int use_overlap;                                   // MS_WGRAD_OVERLAP (default 1; MADNet only, off while profiling)
+    // with the dgrad chain (fork / join through events; inside the captured step this becomes a parallel graph branch).
+    // MADNet only, and off while profiling
     cudaStream_t wstream; cudaEvent_t ev_fork, ev_join; bool wstream_dirty;
     int fork_wgrad(cudaStream_t st, cudaStream_t* ws);
     int join_wgrad(cudaStream_t st);
     int backward_impl(int mode, int group, cudaStream_t st);
     int run(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st);
     int run_eager(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st);
-    // ---- split-16-bit wgmma path (conv_bf.cu), the default implementation of every eligible conv / dgrad
-    int use_stem;                                  // direct CUDA-core kernels for DispNet conv1 (MS_STEM=0: tensor-core path)
-    int use_bf_wgrad;                              // split-bf16 weight gradients (MS_BF_WGRAD=0: the fp32 CUDA-core kernels)
-    int use_heads;                                 // direct kernels for the 3x3 -> 1 heads (MS_HEADS=0: generic path)
-    int conv_impl;                                 // 1 = split-16-bit tensor cores (default), 0 = fp32 CUDA-core kernels (MS_CONV_IMPL=fp32)
+    // ---- split-16-bit wgmma path (conv_bf.cu): every eligible conv / dgrad / weight gradient
     std::map<const float*, ActPlanes> planes;      // bf16 hi/lo planes of tensors that feed convolutions (key: base pointer)
     std::set<const float*> fresh;                  // planes already written by a conv_bf epilogue in the current pass
     struct BfW { void* tiles; bool ok; };
@@ -105,7 +100,7 @@ struct Engine {
     float* bf_part; unsigned int* bf_tickets;
     void add_planes(Bump& A, const TView& v, int fmt);      // fmt 1 = forward activation (fp16 of x/16), 0 = gradient (bf16)
     ActPlanes wg_xp; size_t wg_xp_halfs;              // bf16 scratch planes: forward activations re-split for the weight gradient
-    float act_scale;                                  // power-of-two scale of the fp16 forward planes (per network, MS_ACT_SCALE overrides)
+    float act_scale;                                  // power-of-two scale of the fp16 forward planes (per network)
     const ActPlanes* planes_of(const TView& v) const;
     int ensure_planes(const TView& v, cudaStream_t st);
     // ---- data-parallel exchange over NVLink peer memory (csrc/dp.cu)

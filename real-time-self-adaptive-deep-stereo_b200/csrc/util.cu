@@ -1,7 +1,5 @@
 #include "common.cuh"
-#include <cstdlib>
 #include <mutex>
-#include <set>
 namespace ms {
 static std::mutex g_mu;
 static std::string g_err;
@@ -9,22 +7,7 @@ void set_error(const std::string& s) { std::lock_guard<std::mutex> l(g_mu); g_er
 const char* last_error_cstr() { std::lock_guard<std::mutex> l(g_mu); return g_err.c_str(); }
 static bool g_pdl_suppressed = false;
 void pdl_set_suppressed(bool s) { g_pdl_suppressed = s; }
-bool pdl_enabled() {
-    if (g_pdl_suppressed) return false;
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("MS_PDL"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v != 0;
-}
-void carveout_once(const void* kernel) {
-    static int on = -1;
-    if (on < 0) { const char* e = getenv("MS_CARVEOUT"); on = (e && e[0] == '1') ? 1 : 0; }
-    if (!on) return;
-    static std::set<const void*> seen;
-    std::lock_guard<std::mutex> l(g_mu);
-    if (!seen.insert(kernel).second) return;
-    (void)cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    (void)cudaGetLastError();
-}
+bool pdl_enabled() { return !g_pdl_suppressed; }
 static long long g_launches = 0;
 long long launch_count() { return g_launches; }
 void add_launches(long long n) { g_launches += n; }
