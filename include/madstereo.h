@@ -167,6 +167,15 @@ int ms_reproj_loss(const float* left, const float* right, const float* disp, int
 int ms_momentum_update(float* w, const float* g, float* m, size_t n, float lr, float mu, float grad_scale,
                        void* stream);
 
+/* Replaces tf.train.AdamOptimizer(lr) (Demo/demo_model.py:163) applied to one var_list, with TF1's ApplyAdam semantics:
+ *   g = grad * grad_scale ; lr_t = lr * sqrt(1 - beta2_power) / (1 - beta1_power)
+ *   m += (g - m) * (1 - beta1) ; v += (g*g - v) * (1 - beta2) ; w -= lr_t * m / (eps + sqrt(v))
+ * then (what the optimizer's _finish does after the train op) beta1_power *= beta1, beta2_power *= beta2 in fp32.
+ * powers: device float[2] = {beta1_power, beta2_power}, start {beta1, beta2}; read and advanced on the device, so the call
+ * can be captured into a CUDA graph.  w, g, m, v: 16-byte aligned. */
+int ms_adam_update(float* w, const float* g, float* m, float* v, float* powers, size_t n, float lr, float beta1, float beta2,
+                   float eps, float grad_scale, void* stream);
+
 /* Replaces preprocessing.pad_image REFLECT padding (Data_utils/preprocessing.py:7-29). */
 int ms_pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int Hp, int Wp, int dst_cs,
                    float scale, float bias, void* stream);
@@ -194,6 +203,20 @@ int ms_engine_set_input(void* e, const float* left, const float* right, void* st
 /* the same with uint8 frames [B,H,W,3] (host or device): what the reference's decode ops deliver before tf.cast
  * (Data_utils/data_reader.py); converted to fp32 on the device.  Any B, H, W (B*H*W*3 need not be a multiple of 4). */
 int ms_engine_set_input_u8(void* e, const unsigned char* left, const unsigned char* right, void* stream);
+/* Live-demo input (Demo/demo_model.py:72-86: preprocessing.rescale_image + tf.image.resize_image_with_crop_or_pad): uint8
+ * DEVICE frames [B,src_h,src_w,3] at camera size, legacy-bilinear rescaled to (resize_h, resize_w) (align_corners=False, no
+ * half-pixel centres), then centre-cropped (offset floor((r - H) / 2)) or zero-padded (floor((H - r) / 2) before) to the
+ * engine's [B,H,W,3]; kept in fp32.  resize == src means no rescale, and with src == (H, W) the result equals
+ * ms_engine_set_input_u8 bit for bit. */
+int ms_engine_set_input_u8_resized(void* e, const unsigned char* left, const unsigned char* right, int src_h, int src_w,
+                                   int resize_h, int resize_w, void* stream);
+/* Optimizer of ms_engine_update / ms_engine_run (with_update=1).  kind 0 = tf.train.MomentumOptimizer (default,
+ * Stereo_Online_Adaptation.py:85), 1 = tf.train.AdamOptimizer (Demo/demo_model.py:163) as ms_adam_update describes:
+ * m lives in the momentum arena, v_arena holds n_param_floats floats (16-byte aligned), powers is a device float[2]
+ * {beta1_power, beta2_power} that every train op shares and advances on the device.  Caller-owned, like the other arenas.
+ * Changing the optimizer drops the captured step graphs.  Under Adam, with_update=2 is refused (the fused data-parallel
+ * exchange applies momentum only). */
+int ms_engine_set_optimizer(void* e, int kind, float beta1, float beta2, float eps, float* v_arena, float* powers);
 int ms_engine_set_gt(void* e, const float* gt, void* stream);
 /* Continual-adaptation variant (reference Stereo_Continual_Adaptation.py:75,112,133; Losses/loss_factory.py:304-351
  * get_proxy_loss('mean_l1')): proxy disparities [B,H,W,1] (host or device) and the loss selector.  kind 0 = reprojection

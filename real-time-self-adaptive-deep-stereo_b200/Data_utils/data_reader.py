@@ -80,6 +80,16 @@ def read_image_from_disc(image_path):
     return np.ascontiguousarray(img[:, :, :3])
 
 
+def read_image_u8_from_disc(image_path):
+    """uint8 [H,W,3] RGB: the decoded image before the cast of read_image_from_disc (what a camera delivers)."""
+    img = _imread(image_path)
+    if img.dtype != np.uint8:
+        raise Exception('%s is not an 8-bit image' % image_path)
+    if img.shape[2] == 1:
+        img = np.repeat(img, 3, axis=2)
+    return np.ascontiguousarray(img[:, :, :3])
+
+
 def read_gt_from_disc(gt_path):
     """float32 [H,W,1]: PFM as is; 16-bit PNG / 256; 8-bit PNG as is."""
     if gt_path.lower().endswith('pfm'):

@@ -50,6 +50,32 @@ def load_weights(ckpt_path, variables, mask=[], prefix="", ignore_list=[]):
     return {var: get(key) for key, var in mapping.items()}
 
 
+def load_adam_state(ckpt_path, trained_variables, beta1=0.9, beta2=0.999, prefix="", ignore_list=[]):
+    """Adam optimizer state of the demo's graph (Demo/demo_model.py:163), as the demo's restore assigns it: a default
+    tf.train.Saver() (Train.py) also saves `<var>/Adam` (m), `<var>/Adam_1` (v), `beta1_power` and `beta2_power`, and
+    get_var_to_restore_list matches every global variable the checkpoint names.
+
+    trained_variables: {variable name: shape} of the variables some train op trains (slots exist only for those).
+    -> {'m': {var: array}, 'v': {var: array}, 'powers': (beta1_power, beta2_power) or None (nothing is trained),
+        'found': number of matching checkpoint entries}.  Entries the checkpoint lacks start at zero / (beta1, beta2)."""
+    names = list(trained_variables)
+    wanted = [n + '/Adam' for n in names] + [n + '/Adam_1' for n in names]
+    if names:
+        wanted += ['beta1_power', 'beta2_power']
+    mapping = get_var_to_restore_list(ckpt_path, [], prefix, ignore_list, wanted)
+    _shapes, get = _open(ckpt_path)
+    found = {var: np.asarray(get(key), dtype=np.float32) for key, var in mapping.items()}
+    state = {'m': {}, 'v': {}, 'powers': None, 'found': len(found)}
+    for n in names:
+        shape = tuple(trained_variables[n])
+        state['m'][n] = found[n + '/Adam'].reshape(shape) if n + '/Adam' in found else np.zeros(shape, np.float32)
+        state['v'][n] = found[n + '/Adam_1'].reshape(shape) if n + '/Adam_1' in found else np.zeros(shape, np.float32)
+    if names:
+        state['powers'] = (float(found['beta1_power']) if 'beta1_power' in found else float(np.float32(beta1)),
+                           float(found['beta2_power']) if 'beta2_power' in found else float(np.float32(beta2)))
+    return state
+
+
 def latest_checkpoint(logdir):
     """tf.train.latest_checkpoint: the prefix named by `<logdir>/checkpoint` (model_checkpoint_path: "...")."""
     state = os.path.join(logdir, 'checkpoint')

@@ -373,6 +373,11 @@ int ms_momentum_update(float* w, const float* g, float* m, size_t n, float lr, f
     return momentum_update(w, g, m, n, lr, mu, grad_scale, S(stream));
 }
 
+int ms_adam_update(float* w, const float* g, float* m, float* v, float* powers, size_t n, float lr, float beta1, float beta2,
+                   float eps, float grad_scale, void* stream) {
+    return adam_update(w, g, m, v, powers, n, lr, beta1, beta2, eps, grad_scale, S(stream));
+}
+
 int ms_pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int Hp, int Wp, int dst_cs, float scale,
                    float bias, void* stream) {
     return pad_reflect(src, B, H, W, C, dst, Hp, Wp, dst_cs, scale, bias, S(stream));
@@ -459,6 +464,13 @@ int ms_engine_set_input(void* h, const float* left, const float* right, void* st
 }
 int ms_engine_set_input_u8(void* h, const unsigned char* left, const unsigned char* right, void* stream) {
     return static_cast<Engine*>(h)->set_input_u8(left, right, S(stream));
+}
+int ms_engine_set_input_u8_resized(void* h, const unsigned char* left, const unsigned char* right, int src_h, int src_w,
+                                   int resize_h, int resize_w, void* stream) {
+    return static_cast<Engine*>(h)->set_input_u8_resized(left, right, src_h, src_w, resize_h, resize_w, S(stream));
+}
+int ms_engine_set_optimizer(void* h, int kind, float beta1, float beta2, float eps, float* v_arena, float* powers) {
+    return static_cast<Engine*>(h)->set_optimizer(kind, beta1, beta2, eps, v_arena, powers);
 }
 int ms_engine_set_gt(void* h, const float* gt, void* stream) {
     Engine* e = static_cast<Engine*>(h);

@@ -182,6 +182,9 @@ int add_channels(float* dst, int dcs, const float* src, int scs, size_t pixels, 
                  int accumulate, cudaStream_t st);
 int fill(float* p, size_t n, float v, cudaStream_t st);
 int u8_to_f32(const unsigned char* src, float* dst, size_t n, cudaStream_t st);
+// uint8 [B,h,w,3] left + right frames -> fp32 [B,H,W,3]: legacy bilinear rescale to (rh, rw), then centre crop / zero pad
+int u8_resize_crop(const unsigned char* left, const unsigned char* right, int B, int h, int w, int rh, int rw, float* dst_left,
+                   float* dst_right, int H, int W, cudaStream_t st);
 
 // loss (loss.cu)
 struct ReprojLoss {
@@ -203,6 +206,9 @@ int proxy_loss(const float* disp, const float* proxy, int n, float weight, float
 // optimizer (optim.cu)
 int momentum_update(float* w, const float* g, float* m, size_t n, float lr, float mu, float gscale,
                     cudaStream_t st);
+// Adam over w/g/m/v arenas; powers = device [beta1_power, beta2_power], read by the update and then advanced once
+int adam_update(float* w, const float* g, float* m, float* v, float* powers, size_t n, float lr, float b1, float b2, float eps,
+                float gscale, cudaStream_t st);
 
 }  // namespace ms
 

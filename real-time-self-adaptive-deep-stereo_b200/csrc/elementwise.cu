@@ -254,4 +254,51 @@ int u8_to_f32(const unsigned char* src, float* dst, size_t n, cudaStream_t st) {
     return check_launch("u8_to_f32");
 }
 
+// Camera frames of any size -> the engine's fp32 input, as the live demo builds it (reference Demo/demo_model.py:80-86):
+// preprocessing.rescale_image = tf.image.resize_images legacy bilinear to (rh, rw), then
+// tf.image.resize_image_with_crop_or_pad to (H, W) -- per axis a centre crop at offset floor((r - H) / 2) or a zero pad of
+// floor((H - r) / 2) before.  One thread per output pixel of either frame (left: first B*H*W threads); the result stays
+// fp32 (the demo's loss sees the interpolated values).  rh, rw == h, w is exact: every lerp weight is 0.
+__global__ void u8_resize_crop_kernel(const unsigned char* __restrict__ left, const unsigned char* __restrict__ right, int B,
+                                      int h, int w, int rh, int rw, int oy0, int ox0, float ys, float xs,
+                                      float* __restrict__ dl, float* __restrict__ dr, int H, int W) {
+    pdl_prologue();
+    const size_t per = (size_t)B * H * W;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 2 * per) return;
+    const bool is_r = i >= per;
+    const size_t j = is_r ? i - per : i;
+    const int x = (int)(j % W);
+    const size_t q = j / W;
+    const int y = (int)(q % H), b = (int)(q / H);
+    float* d = (is_r ? dr : dl) + j * 3;
+    const int ry = y + oy0, rx = x + ox0;
+    if (ry < 0 || ry >= rh || rx < 0 || rx >= rw) { d[0] = 0.f; d[1] = 0.f; d[2] = 0.f; return; }
+    const unsigned char* s = (is_r ? right : left) + (size_t)b * h * w * 3;
+    const Lerp ly = lerp_coeff(ry, ys, h), lx = lerp_coeff(rx, xs, w);
+    const unsigned char* t0 = s + ((size_t)ly.i0 * w) * 3;
+    const unsigned char* t1 = s + ((size_t)ly.i1 * w) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float tl = t0[lx.i0 * 3 + c], tr = t0[lx.i1 * 3 + c];
+        const float bl = t1[lx.i0 * 3 + c], br = t1[lx.i1 * 3 + c];
+        const float top = tl + (tr - tl) * lx.f;
+        const float bot = bl + (br - bl) * lx.f;
+        d[c] = top + (bot - top) * ly.f;
+    }
+}
+
+int u8_resize_crop(const unsigned char* left, const unsigned char* right, int B, int h, int w, int rh, int rw, float* dst_left,
+                   float* dst_right, int H, int W, cudaStream_t st) {
+    MS_REQUIRE(B >= 1 && h >= 1 && w >= 1 && rh >= 1 && rw >= 1 && H >= 1 && W >= 1, "u8_resize_crop: bad geometry");
+    MS_REQUIRE(left && right && dst_left && dst_right, "u8_resize_crop: null pointer");
+    const int oy0 = rh >= H ? (rh - H) / 2 : -((H - rh) / 2);
+    const int ox0 = rw >= W ? (rw - W) / 2 : -((W - rw) / 2);
+    const float ys = (float)h / (float)rh, xs = (float)w / (float)rw;     // TF: in / out in fp32, src = dst * scale
+    const size_t total = 2 * (size_t)B * H * W;
+    launch_k(u8_resize_crop_kernel, dim3((unsigned)cdivz(total, 256)), dim3(256), 0, st, left, right, B, h, w, rh, rw, oy0, ox0,
+             ys, xs, dst_left, dst_right, H, W);
+    return check_launch("u8_resize_crop");
+}
+
 }  // namespace ms

@@ -45,6 +45,27 @@ Engine::Engine()
     act_scale = 0.f;
     bf_jobs_dev = nullptr; bf_max_total = 0; bf_part = nullptr; bf_tickets = nullptr;
     dp_rank = 0; dp_world = 1; dp_connected = false; dp_xbuf = nullptr; dp_state = nullptr; dp_cap_floats = 0;
+    opt_kind = 0; adam_b1 = adam_b2 = adam_eps = 0.f; adam_v = nullptr; adam_powers = nullptr;
+}
+
+void Engine::drop_graphs() {
+    for (auto& g : graphs) cudaGraphExecDestroy(g.second.exec);
+    graphs.clear();
+}
+
+int Engine::set_optimizer(int kind, float beta1, float beta2, float eps, float* v, float* powers) {
+    MS_REQUIRE(kind == 0 || kind == 1, "set_optimizer: kind must be 0 (momentum) or 1 (adam)");
+    if (kind == 1) {
+        MS_REQUIRE(v && powers, "set_optimizer: Adam needs the second-moment arena and the two beta powers");
+        MS_REQUIRE((reinterpret_cast<uintptr_t>(v) & 15) == 0, "set_optimizer: the second-moment arena must be 16B aligned");
+        MS_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps >= 0.f, "set_optimizer: bad Adam constants");
+    } else {
+        beta1 = beta2 = eps = 0.f; v = nullptr; powers = nullptr;
+    }
+    if (kind != opt_kind || beta1 != adam_b1 || beta2 != adam_b2 || eps != adam_eps || v != adam_v || powers != adam_powers)
+        drop_graphs();          // the update kernels are baked into the step graphs
+    opt_kind = kind; adam_b1 = beta1; adam_b2 = beta2; adam_eps = eps; adam_v = v; adam_powers = powers;
+    return 0;
 }
 
 void Engine::add_planes(Bump& A, const TView& v, int fmt) {
@@ -522,6 +543,13 @@ int Engine::set_input_u8(const unsigned char* left, const unsigned char* right, 
     return u8_to_f32(right_stage, rr.p, n, st);
 }
 
+// uint8 device frames [B,h,w,3] at camera size: rescale to (rh, rw) and centre crop / zero pad to (H, W) in one pass
+int Engine::set_input_u8_resized(const unsigned char* left, const unsigned char* right, int h, int w, int rh, int rw,
+                                 cudaStream_t st) {
+    MS_REQUIRE(bound, "engine not bound");
+    return u8_resize_crop(left, right, B, h, w, rh, rw, tensors["raw_left"].p, tensors["raw_right"].p, H, W, st);
+}
+
 int Engine::prep_layers(int group, cudaStream_t st) {
     if (bf_jobs.empty()) return 0;
     int b, e;
@@ -809,7 +837,12 @@ int Engine::update(int group, float lr, float mu, float gscale, cudaStream_t st)
     MS_REQUIRE(bound, "engine not bound");
     size_t b = 0, e = n_params;
     if (group >= 0) { MS_REQUIRE(group < n_groups, "update: bad group"); b = group_begin[group]; e = group_end[group]; }
-    if (momentum_update(Wt + b, Gr + b, Mo + b, e - b, lr, mu, gscale, st)) return -1;
+    if (opt_kind == 1) {
+        if (adam_update(Wt + b, Gr + b, Mo + b, adam_v + b, adam_powers, e - b, lr, adam_b1, adam_b2, adam_eps, gscale, st))
+            return -1;
+    } else if (momentum_update(Wt + b, Gr + b, Mo + b, e - b, lr, mu, gscale, st)) {
+        return -1;
+    }
     return prep_layers(group, st);      // refresh the tf32 hi/lo copies of exactly the weights that moved
 }
 
@@ -841,6 +874,8 @@ int Engine::run_eager(int mode, int group, int disp_mask, int with_update, float
 int Engine::run(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st) {
     MS_REQUIRE(bound, "engine not bound");
     MS_REQUIRE(mode == 0 || mode == 2 || (mode == 1 && group >= 0 && group < n_groups), "run: bad mode/group");
+    MS_REQUIRE(!(with_update == 2 && mode != 0 && opt_kind != 0),
+               "run: the fused data-parallel exchange (with_update=2) applies momentum only; Adam is single-GPU");
     if (profiling == 1) return run_eager(mode, group, disp_mask, with_update, lr, mu, gscale, st);
     if (weights_dirty) {                    // load / restore happened: refresh every tf32 copy outside the graph
         if (prep_layers(-1, st)) return -1;

@@ -115,6 +115,11 @@ struct Engine {
     float* rs_tmp; size_t rs_tmp_floats;
     float* loss_ws; size_t loss_ws_floats;
     unsigned char* u8_stage;         // 2 x B*H*W*3 bytes: uint8 input staging (set_input_u8)
+    // optimizer of update(): 0 = momentum SGD (Mo = accumulator), 1 = Adam (Mo = first moment, adam_v = second moment,
+    // adam_powers = device [beta1_power, beta2_power] shared by every train op); caller-owned storage (ms_engine_set_optimizer)
+    int opt_kind;
+    float adam_b1, adam_b2, adam_eps;
+    float* adam_v; float* adam_powers;
     float* scalars;                  // [0]=full loss, [1]=train loss, [2]=epe, [3]=bad3
     float* gt;                       // optional ground truth [B,H,W,1]
     float* proxy;                    // proxy disparities [B,H,W,1] of the continual-adaptation variant (loss_kind 1)
@@ -154,6 +159,9 @@ struct Engine {
 
     int set_input(const float* left, const float* right, cudaStream_t st);
     int set_input_u8(const unsigned char* left, const unsigned char* right, cudaStream_t st);
+    int set_input_u8_resized(const unsigned char* left, const unsigned char* right, int h, int w, int rh, int rw, cudaStream_t st);
+    int set_optimizer(int kind, float beta1, float beta2, float eps, float* v, float* powers);
+    void drop_graphs();
     int forward(int disp_mask, cudaStream_t st);
     int loss(int which, int with_grad, int slot, float grad_scale, cudaStream_t st);
     int backward(int mode, int group, cudaStream_t st);     // mode 1 = MAD(group), 2 = FULL

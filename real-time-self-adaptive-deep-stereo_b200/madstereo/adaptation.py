@@ -28,15 +28,33 @@ def softmax(x):
     return np.exp(x) / np.sum(np.exp(x), axis=0)
 
 
+def trained_variable_names(mode, groups, layers):
+    """TF variable names some train op trains, in layer order: the union of the MAD groups (lists of layer indices), every
+    variable in FULL, none in NONE.  TF creates optimizer slots per var_list of each minimize(), so only these have them.
+    layers: objects with .index, .scope and .bias_name (StereoEngine.layers)."""
+    if mode == 'NONE':
+        return []
+    chosen = None if mode == 'FULL' else {i for g in groups for i in g}
+    names = []
+    for l in layers:
+        if chosen is None or l.index in chosen:
+            names += [l.scope + '/weights', l.scope + '/' + l.bias_name]
+    return names
+
+
 class OnlineAdaptation(object):
     def __init__(self, net, mode='MAD', train_config=None, lr=0.0001, momentum=0.9, sample_mode='SEQUENTIAL',
                  num_blocks=1, fixed_id=0, sample_frequency=1, ssim_th=0.5, process_group=None,
-                 loss='reprojection', decay=0.99, uf=0.01, dilation=1):
+                 loss='reprojection', decay=0.99, uf=0.01, dilation=1, optimizer='momentum', beta1=0.9, beta2=0.999,
+                 epsilon=1e-8):
         """loss='proxy', decay, uf, dilation: the continual-adaptation variant (Stereo_Continual_Adaptation.py): masked L1 to
         proxy disparities (weights 0.01 full-resolution / FULL, 0.1 per MAD module, :75,112), reward recurrence
-        h <- decay*h, h[i] += uf*gain (:232-234), a train op only every `dilation`-th frame (:212)."""
+        h <- decay*h, h[i] += uf*gain (:232-234), a train op only every `dilation`-th frame (:212).
+        optimizer='adam': tf.train.AdamOptimizer(lr) with TF1's defaults, as the live demo adapts (Demo/demo_model.py:163);
+        one pair of bias-correction powers shared by every train op.  Single GPU only."""
         assert mode in ('NONE', 'FULL', 'MAD')
         assert loss in ('reprojection', 'proxy')
+        assert optimizer in ('momentum', 'adam')
         self.loss_kind, self.decay, self.uf, self.dilation = loss, float(decay), float(uf), int(dilation)
         self.net, self.engine, self.mode = net, net.engine, mode
         self.lr, self.mu = float(lr), float(momentum)
@@ -47,6 +65,9 @@ class OnlineAdaptation(object):
         if torch.distributed.is_available() and torch.distributed.is_initialized():
             self.world = torch.distributed.get_world_size(self.pg)
             self.rank = torch.distributed.get_rank(self.pg)
+        if optimizer == 'adam' and self.world > 1:
+            raise MadStereoError("optimizer='adam' runs on a single GPU: the data-parallel exchange applies momentum only")
+        self.optimizer = optimizer
         predictions = net.get_disparities()
         self.groups = []
         if mode == 'MAD':
@@ -66,6 +87,9 @@ class OnlineAdaptation(object):
         self.engine.bind()
         if loss == 'proxy':
             self.engine.set_loss('proxy')
+        if optimizer == 'adam':
+            self.engine.set_optimizer('adam', beta1, beta2, epsilon)
+        self._adam_snapshot = None
         self.num_actions = len(self.groups) if mode == 'MAD' else (1 if mode == 'FULL' else 0)
         self.fetch_counter = [0] * self.num_actions
         self.sample_distribution = np.zeros(shape=[self.num_actions])
@@ -132,11 +156,42 @@ class OnlineAdaptation(object):
         from .tf_checkpoint import write_checkpoint
         write_checkpoint(prefix, self.engine.export_params())
 
+    def trained_variable_names(self):
+        """Variables some train op trains: only these have optimizer slots."""
+        return trained_variable_names(self.mode, self.groups, self.engine.layers)
+
+    def trained_variable_shapes(self):
+        views = self.engine.param_views()
+        return {n: tuple(views[n].shape) for n in self.trained_variable_names()}
+
+    def load_adam_state(self, state):
+        """state: Data_utils.weights_utils.load_adam_state(...) -- {'m': {var: array}, 'v': {var: array},
+        'powers': (beta1_power, beta2_power) or None, 'found': number of checkpoint entries it came from}.  Writes the
+        first moments into the momentum arena, the second moments into the Adam arena and the shared powers.  When the
+        checkpoint held any of them they join the reset snapshot: the demo's reset re-runs the same restore, which
+        assigns every global variable the checkpoint names (Demo/demo_model.py:198-201)."""
+        if self.optimizer != 'adam':
+            raise MadStereoError("load_adam_state needs optimizer='adam'")
+        eng = self.engine
+        mv, vv = eng.param_views(eng.momentum), eng.param_views(eng.adam_v)
+        for name, arr in state['m'].items():
+            mv[name].copy_(torch.as_tensor(np.asarray(arr, dtype=np.float32)).reshape(mv[name].shape))
+        for name, arr in state['v'].items():
+            vv[name].copy_(torch.as_tensor(np.asarray(arr, dtype=np.float32)).reshape(vv[name].shape))
+        if state.get('powers') is not None:
+            eng.adam_powers.copy_(torch.tensor(state['powers'], dtype=torch.float32))
+        if state.get('found', 0) > 0:
+            self._adam_snapshot = (eng.momentum.clone(), eng.adam_v.clone(), eng.adam_powers.clone())
+
     def restore(self):
-        """restorer.restore(sess, weights) (:242-244): weights only; momentum slots are left untouched."""
+        """restorer.restore(sess, weights) (:242-244): weights only; momentum slots are left untouched.  Under Adam the
+        slots and powers are restored too when the checkpoint held them (load_adam_state)."""
         if self._snapshot is None:
             raise MadStereoError('no weight snapshot to restore')
         self.engine.weights.copy_(self._snapshot)
+        if self._adam_snapshot is not None:
+            for dst, src in zip((self.engine.momentum, self.engine.adam_v, self.engine.adam_powers), self._adam_snapshot):
+                dst.copy_(src)
         self.engine.weights_changed()
 
     # ---- one frame ---------------------------------------------------------------------------------
@@ -151,14 +206,18 @@ class OnlineAdaptation(object):
         eng = self.engine
         u8 = eng._is_u8(left) and eng._is_u8(right)
         dt = torch.uint8 if u8 else torch.float32
-        if self._stage is None or self._stage[0].dtype != dt:
-            shape = (eng.B, eng.H, eng.W, 3)
+        resized = u8 and eng.resize_shape is not None     # frames at camera size: staging buffers of the source size
+        if resized:
+            l, r = eng._u8_source(left), eng._u8_source(right)
+        else:
+            l, r = (eng._as_u8(left), eng._as_u8(right)) if u8 else (eng._as_f32(left), eng._as_f32(right))
+        shape = tuple(l.shape) if resized else (eng.B, eng.H, eng.W, 3)
+        if self._stage is None or self._stage[0].dtype != dt or tuple(self._stage[0].shape) != shape:
             self._stage = [torch.empty(shape, dtype=dt, device=eng.device) for _ in range(2)]
             self._copy_stream = torch.cuda.Stream(device=eng.device)
             self._stage_ready = torch.cuda.Event()
             self._stage_free = torch.cuda.Event()
             self._stage_free.record(torch.cuda.current_stream(eng.device))
-        l, r = (eng._as_u8(left), eng._as_u8(right)) if u8 else (eng._as_f32(left), eng._as_f32(right))
         with torch.cuda.stream(self._copy_stream):
             self._copy_stream.wait_event(self._stage_free)      # the previous frame's staging -> input copy is done
             self._stage[0].copy_(l, non_blocking=True)

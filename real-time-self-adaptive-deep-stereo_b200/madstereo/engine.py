@@ -63,6 +63,9 @@ class StereoEngine:
         self.n_groups = 0
         self.bound = False
         self._keep = []
+        self.optimizer = 'momentum'
+        self.resize_shape = None      # set_resize(): None = uint8 frames must be [B,H,W,3]; else (rh, rw), -1 = no rescale
+        self._rs_stage = None
 
     def _on_device(self):
         """Context that makes this engine's GPU current -- a no-op object when it already is (the per-frame calls of a
@@ -146,7 +149,11 @@ class StereoEngine:
 
     # ---- per-frame calls ---------------------------------------------------------------------
     def set_input(self, left, right):
-        """left/right: [B,H,W,3] float32 torch tensors (CUDA, or pinned/pageable CPU) or numpy arrays."""
+        """left/right: [B,H,W,3] float32 torch tensors (CUDA, or pinned/pageable CPU) or numpy arrays.  After set_resize(),
+        uint8 frames [B,h,w,3] of any size are rescaled and centre-cropped / zero-padded to [B,H,W,3] on the device."""
+        if self.resize_shape is not None and self._is_u8(left) and self._is_u8(right):
+            self._set_input_resized(left, right)
+            return
         if self._is_u8(left) and self._is_u8(right):
             l, r = self._as_u8(left), self._as_u8(right)
             self._keep = [l, r]
@@ -157,6 +164,67 @@ class StereoEngine:
         self._keep = [l, r]
         with self._on_device():
             check(self._lib.ms_engine_set_input(self._h, _ptr(l), _ptr(r), _stream()), 'set_input')
+
+    def set_resize(self, image_shape=(-1, -1)):
+        """Accept uint8 frames of any size from now on, as the live demo feeds them (Demo/demo_model.py:80-86): a legacy
+        bilinear rescale to image_shape = (rh, rw) (tf.image.resize_images, align_corners=False), then
+        tf.image.resize_image_with_crop_or_pad to the engine's (H, W).  (-1, -1) skips the rescale; None turns the
+        geometry off again (uint8 frames must then be exactly [B,H,W,3])."""
+        if image_shape is not None:
+            image_shape = tuple(int(v) for v in image_shape)
+            if len(image_shape) != 2 or (min(image_shape) < 1 and image_shape != (-1, -1)):
+                raise MadStereoError('set_resize: image_shape must be (height, width) or (-1, -1), got %r' % (image_shape,))
+        self.resize_shape = image_shape
+
+    def _u8_source(self, x):
+        """uint8 [B,h,w,3] frame -> contiguous CUDA tensor on this engine's device (host frames are copied on the current
+        stream into a staging buffer of the source size; pinned ones asynchronously)."""
+        if isinstance(x, np.ndarray):
+            x = torch.from_numpy(np.ascontiguousarray(x))
+        if x.dim() != 4 or x.shape[0] != self.B or x.shape[3] != 3:
+            raise MadStereoError('input shape %s is not [%d,h,w,3]' % (tuple(x.shape), self.B))
+        if x.is_cuda and x.device != self.device:
+            raise MadStereoError('input on %s, engine on %s' % (x.device, self.device))
+        return x.contiguous()
+
+    def _set_input_resized(self, left, right):
+        l, r = self._u8_source(left), self._u8_source(right)
+        if tuple(l.shape) != tuple(r.shape):
+            raise MadStereoError('left %s and right %s frames differ in size' % (tuple(l.shape), tuple(r.shape)))
+        h, w = int(l.shape[1]), int(l.shape[2])
+        rh, rw = (h, w) if self.resize_shape == (-1, -1) else self.resize_shape
+        self._keep_host = [l, r]              # a pinned source must outlive its asynchronous copy
+        if not l.is_cuda or not r.is_cuda:
+            shape = (2,) + tuple(l.shape)
+            if self._rs_stage is None or tuple(self._rs_stage.shape) != shape:
+                self._rs_stage = torch.empty(shape, dtype=torch.uint8, device=self.device)
+            self._rs_stage[0].copy_(l, non_blocking=l.is_pinned())
+            self._rs_stage[1].copy_(r, non_blocking=r.is_pinned())
+            l, r = self._rs_stage[0], self._rs_stage[1]
+        self._keep = [l, r]
+        with self._on_device():
+            check(self._lib.ms_engine_set_input_u8_resized(self._h, _ptr(l), _ptr(r), h, w, rh, rw, _stream()),
+                  'set_input_u8_resized')
+
+    def set_optimizer(self, kind, beta1=0.9, beta2=0.999, epsilon=1e-8):
+        """'momentum' (tf.train.MomentumOptimizer, the default) or 'adam' (tf.train.AdamOptimizer, Demo/demo_model.py:163).
+        Adam keeps its first moment in the momentum arena, its second moment in `adam_v` and the shared bias-correction
+        powers [beta1_power, beta2_power] in `adam_powers` (start: beta1, beta2; advanced on the device by every update).
+        Changing the optimizer drops the captured step graphs."""
+        if not self.bound:
+            raise MadStereoError('set_optimizer: bind() first')
+        if kind == 'momentum':
+            check(self._lib.ms_engine_set_optimizer(self._h, 0, 0.0, 0.0, 0.0, c_void_p(0), c_void_p(0)), 'set_optimizer')
+        elif kind == 'adam':
+            if getattr(self, 'adam_v', None) is None:
+                self.adam_v = torch.zeros(self.n_params, dtype=torch.float32, device=self.device)
+                self.adam_powers = torch.tensor([beta1, beta2], dtype=torch.float32, device=self.device)
+            check(self._lib.ms_engine_set_optimizer(self._h, 1, beta1, beta2, epsilon, _ptr(self.adam_v),
+                                                    _ptr(self.adam_powers)), 'set_optimizer')
+            self.adam_betas = (float(beta1), float(beta2), float(epsilon))
+        else:
+            raise MadStereoError("set_optimizer: kind must be 'momentum' or 'adam', got %r" % (kind,))
+        self.optimizer = kind
 
     @staticmethod
     def _is_u8(x):
