@@ -26,8 +26,14 @@
 //   * split-K over (K block, patch) units for small maps; the last-arriving CTA of a tile reduces the partial
 //     sums in fixed order (deterministic) and runs the epilogue -- no separate reduce launch.
 //
+//   * narrow layers (output channels rounded up to CN = 16, 32, 64 or 96) keep the GEMM the other way round instead
+//     ("pixel-major"): M = pixels (64 consecutive patch pixels per m64 MMA), N = CN channels of a CN-row weight tile.
+//     The swap-AB tile would issue 128 / CN times the MMAs the layer needs, on zero weight rows.  A tap is still a row
+//     offset into the halo patch, and a 64-pixel block a further 64 rows (eight whole swizzle atoms).
+//
 // Warpgroup roles (384 threads): warpgroup 0 = TMA producer (one warp issues), warpgroups 1-2 = wgmma on output channels
-// [0, 64) / [64, 128) of the M block, then the epilogue.
+// [0, 64) / [64, 128) of the M block (pixel-major: on pixels [0, N/2) / [N/2, N) of the tile, or, for a 64-pixel tile, on
+// channels [0, CN/2) / [CN/2, CN)), then the epilogue.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -48,6 +54,9 @@ constexpr int BF_MAX_PATCH = 16;
 constexpr int BF_MAX_TAPS = 49;
 constexpr int BF_STAGE_LD = 132;     // floats per pixel row of the epilogue staging tile (128 channels + 4: no bank conflicts)
 
+// output channels of one weight tile (= one CTA): Mpad itself for the narrow widths 16 / 32 / 64 / 96, else 128
+__host__ __device__ __forceinline__ int bf_tile_rows(int Mpad) { return Mpad < 128 ? Mpad : 128; }
+
 struct BfPatch { short dx, dy, ntaps, tap0; };
 struct BfTap { short row_off, widx; };
 
@@ -61,7 +70,7 @@ struct ConvBfParams {
     int kch;                      // channels per K block: 32 (64-byte rows, SWIZZLE_64B) or 64 (128-byte rows, SWIZZLE_128B)
     int taps_total;
     uint32_t slot_bytes;          // bytes of one patch plane in shared memory
-    uint32_t wtile_bytes;         // bytes of one weight tile plane (128 rows x kch x 2)
+    uint32_t wtile_bytes;         // bytes of one weight tile plane (bf_tile_rows(Mpad) rows x kch x 2)
     int NP, NW;
     int fmt;                      // operand format: 0 = bf16 planes, 1 = fp16 planes (activation planes hold x * scale)
     float acc_scale;              // multiplies the accumulator (1 / scale of the input planes, a power of two: exact)
@@ -99,8 +108,9 @@ __device__ __forceinline__ void split16(float v, int fmt, float scale, unsigned 
     }
 }
 
-// N: pixels per CTA (64, 96 or 128); BF: 1 = bf16 operand planes, 0 = fp16
-template <int N, int BF>
+// N: pixels per CTA (swap AB: 64, 96 or 128; pixel-major: 64, 128 or 256); BF: 1 = bf16 operand planes, 0 = fp16;
+// CN: 0 = swap AB (128 output channels per CTA), 16 / 32 / 64 / 96 = pixel-major with CN output channels per CTA
+template <int N, int BF, int CN>
 __global__ void __launch_bounds__(BF_THREADS, 1)
 conv_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant__ CUtensorMap mapXl,
                const __grid_constant__ ConvBfParams p) {
@@ -168,12 +178,22 @@ conv_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant_
         return;
     }
 
-    // ================= MMA warpgroups: channels [64 * mg, 64 * mg + 64) of the M block, all N pixels =================
+    // ================= MMA warpgroups: channels [64 * mg, 64 * mg + 64) of the M block, all N pixels (pixel-major: pixel
+    //                   blocks [PB * mg, PB * mg + PB) of 64 and all CN channels, or, for N = 64, all pixels and channels
+    //                   [WN * mg, WN * mg + WN)) =================
+    constexpr int MT = CN ? CN : 128;                         // output channels per CTA
+    constexpr int LD = CN ? CN + 4 : BF_STAGE_LD;             // floats per pixel row of the staging tile
+    constexpr bool CSPLIT = CN && N == 64;                    // pixel-major, one m64 pixel block: the warpgroups split the channels
+    constexpr int WN = CSPLIT ? CN / 2 : CN;                  // pixel-major: channels per warpgroup (MMA N)
+    constexpr int PB = CN && !CSPLIT ? N / 128 : 1;           // accumulator blocks per thread (pixel-major: m64 pixel blocks)
+    constexpr int AR = CN ? WN / 2 : N / 2;                   // registers per accumulator block
     const int mg = (warp >> 2) - 1;
     const int ct = threadIdx.x - 128;                         // 0..255 over both MMA warpgroups
-    float acc_x[N / 2], acc_m[N / 2];                         // cross terms (w_lo*x_hi + w_hi*x_lo) and w_hi*x_hi
+    float acc_x[PB][AR], acc_m[PB][AR];                       // cross terms (w_lo*x_hi + w_hi*x_lo) and w_hi*x_hi
 #pragma unroll
-    for (int i = 0; i < N / 2; ++i) { acc_x[i] = 0.f; acc_m[i] = 0.f; }
+    for (int b = 0; b < PB; ++b)
+#pragma unroll
+        for (int i = 0; i < AR; ++i) { acc_x[b][i] = 0.f; acc_m[b][i] = 0.f; }
     {
         const bool sw128 = p.kch == 64;
         const uint32_t row_unit = (uint32_t)p.kch * 2u;       // bytes of one K-major row (one pixel / one channel)
@@ -191,20 +211,39 @@ conv_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant_
             for (int t = pt.tap0; t < pt.tap0 + pt.ntaps; ++t) {
                 mb_wait(&wfull[ws], wph);
                 const uint32_t boff = (uint32_t)p.tap[t].row_off * row_bytes;
-                const uint64_t xh = wg_desc(pb + boff, 16u, sbo, sw128), xl = wg_desc(pb + p.slot_bytes + boff, 16u, sbo, sw128);
-                const uint32_t wb = base + w_off + (uint32_t)ws * wslot + (uint32_t)mg * 64u * row_unit;
-                const uint64_t wh = wg_desc(wb, 16u, sbo, sw128), wl = wg_desc(wb + p.wtile_bytes, 16u, sbo, sw128);
-                wg_fence_acc(acc_x); wg_fence_acc(acc_m);
+#pragma unroll
+                for (int b = 0; b < PB; ++b) { wg_fence_acc(acc_x[b]); wg_fence_acc(acc_m[b]); }
                 wg_fence();
-                for (int j = 0; j < k16; ++j) {                // K = 16 elements = 32 bytes inside the swizzle row
-                    const uint64_t o = (uint64_t)(j * 2);
-                    Wgmma<N, BF, 0, 0>::mma(acc_x, wl + o, xh + o);
-                    Wgmma<N, BF, 0, 0>::mma(acc_x, wh + o, xl + o);
-                    Wgmma<N, BF, 0, 0>::mma(acc_m, wh + o, xh + o);
+                if constexpr (CN == 0) {
+                    const uint64_t xh = wg_desc(pb + boff, 16u, sbo, sw128), xl = wg_desc(pb + p.slot_bytes + boff, 16u, sbo, sw128);
+                    const uint32_t wb = base + w_off + (uint32_t)ws * wslot + (uint32_t)mg * 64u * row_unit;
+                    const uint64_t wh = wg_desc(wb, 16u, sbo, sw128), wl = wg_desc(wb + p.wtile_bytes, 16u, sbo, sw128);
+                    for (int j = 0; j < k16; ++j) {            // K = 16 elements = 32 bytes inside the swizzle row
+                        const uint64_t o = (uint64_t)(j * 2);
+                        Wgmma<N, BF, 0, 0>::mma(acc_x[0], wl + o, xh + o);
+                        Wgmma<N, BF, 0, 0>::mma(acc_x[0], wh + o, xl + o);
+                        Wgmma<N, BF, 0, 0>::mma(acc_m[0], wh + o, xh + o);
+                    }
+                } else {
+                    const uint32_t xb = pb + boff + (CSPLIT ? 0u : (uint32_t)(mg * PB) * 64u * row_unit);
+                    const uint32_t wb = base + w_off + (uint32_t)ws * wslot + (CSPLIT ? (uint32_t)(mg * WN) * row_unit : 0u);
+                    const uint64_t wh = wg_desc(wb, 16u, sbo, sw128), wl = wg_desc(wb + p.wtile_bytes, 16u, sbo, sw128);
+                    for (int j = 0; j < k16; ++j) {
+                        const uint64_t o = (uint64_t)(j * 2);
+#pragma unroll
+                        for (int b = 0; b < PB; ++b) {
+                            const uint32_t xa = xb + (uint32_t)b * 64u * row_unit;
+                            const uint64_t xh = wg_desc(xa, 16u, sbo, sw128) + o, xl = wg_desc(xa + p.slot_bytes, 16u, sbo, sw128) + o;
+                            Wgmma<WN, BF, 0, 0>::mma(acc_x[b], xh, wl + o);
+                            Wgmma<WN, BF, 0, 0>::mma(acc_x[b], xl, wh + o);
+                            Wgmma<WN, BF, 0, 0>::mma(acc_m[b], xh, wh + o);
+                        }
+                    }
                 }
                 wg_commit();
                 wg_wait<1>();                                 // the previous tap's MMAs are done with their operands
-                wg_fence_acc(acc_x); wg_fence_acc(acc_m);
+#pragma unroll
+                for (int b = 0; b < PB; ++b) { wg_fence_acc(acc_x[b]); wg_fence_acc(acc_m[b]); }
                 if (lane == 0) {
                     if (pend_w >= 0) mb_arrive(&wempty[pend_w]);
                     if (pend_p >= 0) mb_arrive(&pempty[pend_p]);
@@ -217,30 +256,44 @@ conv_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant_
             if (++pi == p.n_patches) pi = 0;
         }
         wg_wait<0>();
-        wg_fence_acc(acc_x); wg_fence_acc(acc_m);
+#pragma unroll
+        for (int b = 0; b < PB; ++b) { wg_fence_acc(acc_x[b]); wg_fence_acc(acc_m[b]); }
     }
 
     // ================= epilogue: accumulators -> staging tile [pixel][channel] in the (now idle) pipeline buffers ==========
     float* const stage = reinterpret_cast<float*>(gbase);
     named_sync(1, 256);                                       // both warpgroups' MMAs have finished reading the rings
     {
-        const int row = mg * 64 + (warp & 3) * 16 + (lane >> 2);
+        // fragment row (MMA M index) and column pair (MMA N index), wgmma_ptx.cuh
+        const int row = (warp & 3) * 16 + (lane >> 2);
         const int col = 2 * (lane & 3);
+        if constexpr (CN == 0) {                              // rows are channels, columns pixels
 #pragma unroll
-        for (int j = 0; j < N / 8; ++j) {
-            float* s0 = stage + (size_t)(8 * j + col) * BF_STAGE_LD + row;
-            s0[0] = acc_x[4 * j] + acc_m[4 * j];
-            s0[BF_STAGE_LD] = acc_x[4 * j + 1] + acc_m[4 * j + 1];
-            s0[8] = acc_x[4 * j + 2] + acc_m[4 * j + 2];
-            s0[BF_STAGE_LD + 8] = acc_x[4 * j + 3] + acc_m[4 * j + 3];
+            for (int j = 0; j < N / 8; ++j) {
+                float* s0 = stage + (size_t)(8 * j + col) * LD + mg * 64 + row;
+                s0[0] = acc_x[0][4 * j] + acc_m[0][4 * j];
+                s0[LD] = acc_x[0][4 * j + 1] + acc_m[0][4 * j + 1];
+                s0[8] = acc_x[0][4 * j + 2] + acc_m[0][4 * j + 2];
+                s0[LD + 8] = acc_x[0][4 * j + 3] + acc_m[0][4 * j + 3];
+            }
+        } else {                                              // rows are pixels, columns channels
+#pragma unroll
+            for (int b = 0; b < PB; ++b)
+#pragma unroll
+                for (int j = 0; j < WN / 8; ++j) {
+                    float* s0 = stage + (size_t)((CSPLIT ? 0 : (mg * PB + b) * 64) + row) * LD + (CSPLIT ? mg * WN : 0) + 8 * j + col;
+                    *reinterpret_cast<float2*>(s0) = make_float2(acc_x[b][4 * j] + acc_m[b][4 * j], acc_x[b][4 * j + 1] + acc_m[b][4 * j + 1]);
+                    *reinterpret_cast<float2*>(s0 + 8 * LD) =
+                        make_float2(acc_x[b][4 * j + 2] + acc_m[b][4 * j + 2], acc_x[b][4 * j + 3] + acc_m[b][4 * j + 3]);
+                }
         }
     }
     named_sync(1, 256);
 
     // thread <-> 4 consecutive channels of one pixel: 128-bit loads / stores for y, residual, mask and accumulate, 64-bit
     // stores for the two 16-bit planes
-    const int chb = blockIdx.y * 128;
-    const int cpp = min(32, (p.cout - chb + 3) >> 2);         // 4-channel chunks per pixel in this M block
+    const int chb = blockIdx.y * MT;
+    const int cpp = min(MT / 4, (p.cout - chb + 3) >> 2);     // 4-channel chunks per pixel in this M block
     const int twm = p.TW - 1;
     const size_t img_pix = (size_t)img * p.Hout;
     const float acc_scale = p.acc_scale, alpha = p.alpha;
@@ -304,21 +357,21 @@ conv_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant_
     if (p.ksplit == 1) {
         for (int i = ct; i < items; i += 256) {
             const int col = i / cpp, c4 = i - col * cpp;
-            const float4 s = *reinterpret_cast<const float4*>(stage + (size_t)col * BF_STAGE_LD + c4 * 4);
+            const float4 s = *reinterpret_cast<const float4*>(stage + (size_t)col * LD + c4 * 4);
             float v[4] = {s.x, s.y, s.z, s.w};
             finish4(col, c4, v);
         }
         return;
     }
-    // raw partial sums: part[(z * n_tiles + tile) * N + col][128 channels]
+    // raw partial sums: part[(z * n_tiles + tile) * N + col][MT channels]
     const int tile_lin = blockIdx.x * gridDim.y + blockIdx.y;
     const size_t n_tiles = (size_t)gridDim.x * gridDim.y;
     {
-        float* mine = p.part + ((size_t)blockIdx.z * n_tiles + tile_lin) * N * 128;
-        for (int i = ct; i < N * 32; i += 256) {
-            const int col = i >> 5, c4 = i & 31;
-            *reinterpret_cast<float4*>(mine + (size_t)col * 128 + c4 * 4) =
-                *reinterpret_cast<const float4*>(stage + (size_t)col * BF_STAGE_LD + c4 * 4);
+        float* mine = p.part + ((size_t)blockIdx.z * n_tiles + tile_lin) * N * MT;
+        for (int i = ct; i < N * (MT / 4); i += 256) {
+            const int col = i / (MT / 4), c4 = i % (MT / 4);
+            *reinterpret_cast<float4*>(mine + (size_t)col * MT + c4 * 4) =
+                *reinterpret_cast<const float4*>(stage + (size_t)col * LD + c4 * 4);
         }
     }
     __threadfence();
@@ -332,11 +385,11 @@ conv_bf_kernel(const __grid_constant__ CUtensorMap mapXh, const __grid_constant_
     named_sync(1, 256);
     if (!last_flag) return;
     __threadfence();
-    const float* col0 = p.part + (size_t)tile_lin * N * 128;
-    const size_t zstride = n_tiles * (size_t)N * 128;
+    const float* col0 = p.part + (size_t)tile_lin * N * MT;
+    const size_t zstride = n_tiles * (size_t)N * MT;
     for (int i = ct; i < items; i += 256) {
         const int col = i / cpp, c4 = i - col * cpp;
-        const float* src = col0 + (size_t)col * 128 + c4 * 4;
+        const float* src = col0 + (size_t)col * MT + c4 * 4;
         float v[4] = {0.f, 0.f, 0.f, 0.f};
         for (int z = 0; z < p.ksplit; ++z) {                  // fixed order: deterministic
             const float4 a = __ldcg(reinterpret_cast<const float4*>(src + (size_t)z * zstride));
@@ -394,18 +447,19 @@ __global__ void bf_prep_weights_kernel(const BfPrepJob* __restrict__ jobs) {
     pdl_prologue();
     const BfPrepJob j = jobs[blockIdx.y];
     const int kch = j.Kpad > 32 ? 64 : 32;
-    const int kblocks = j.Kpad / kch, mblocks = j.Mpad / 128;
-    const size_t tile = (size_t)128 * kch;                         // elements per tile plane
+    const int rows = bf_tile_rows(j.Mpad);
+    const int kblocks = j.Kpad / kch, mblocks = j.Mpad / rows;
+    const size_t tile = (size_t)rows * kch;                        // elements per tile plane
     const size_t total = (size_t)mblocks * j.taps * kblocks * tile;
     unsigned short* dst = reinterpret_cast<unsigned short*>(j.tiles);
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const int kk = (int)(i % kch);
         size_t q = i / kch;
-        const int r = (int)(q % 128); q /= 128;
+        const int r = (int)(q % rows); q /= rows;
         const int kb = (int)(q % kblocks); q /= kblocks;
         const int t = (int)(q % j.taps);
         const int mb = (int)(q / j.taps);
-        const int m = mb * 128 + r, k = kb * kch + kk;
+        const int m = mb * rows + r, k = kb * kch + kk;
         float v = 0.f;
         if (m < j.M && k < j.K)
             v = j.transposed_src ? j.src[((size_t)t * j.K + k) * j.M + m] : j.src[((size_t)t * j.M + m) * j.K + k];
@@ -434,8 +488,9 @@ int bf_prep_weights(const BfPrepJob* jobs_dev, int njobs, size_t max_total, cuda
     return check_launch("bf_prep_weights");
 }
 
+// M rounds up to 16, 32, 64 or 96 (one pixel-major weight tile of that many rows) or else to a multiple of 128 (swap AB)
 void conv_bf_weight_dims(int M, int K, int& Mpad, int& Kpad) {
-    Mpad = (M + 127) / 128 * 128;
+    Mpad = M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : M <= 96 ? 96 : (M + 127) / 128 * 128;
     Kpad = K > 32 ? (K + 63) / 64 * 64 : 32;
 }
 size_t conv_bf_weight_halfs(int taps, int M, int K) {       // 16-bit elements of the tiled image, both planes
@@ -520,15 +575,23 @@ bool conv_bf_supported(const ConvGemm& g) {
     return true;
 }
 
+typedef void (*BfKernel)(const CUtensorMap, const CUtensorMap, const ConvBfParams);
+struct BfVariant { int N, CN; BfKernel k[2]; };       // k[BF]
+#define MS_BF_VARIANT(N, CN) {N, CN, {conv_bf_kernel<N, 0, CN>, conv_bf_kernel<N, 1, CN>}}
+// pixel-major: N * CN / 128 accumulator registers per thread, at most 128
+static const BfVariant BF_VARIANTS[] = {
+    MS_BF_VARIANT(64, 0), MS_BF_VARIANT(96, 0), MS_BF_VARIANT(128, 0),
+    MS_BF_VARIANT(64, 16), MS_BF_VARIANT(128, 16), MS_BF_VARIANT(256, 16), MS_BF_VARIANT(64, 32), MS_BF_VARIANT(128, 32),
+    MS_BF_VARIANT(256, 32), MS_BF_VARIANT(64, 64), MS_BF_VARIANT(128, 64), MS_BF_VARIANT(256, 64), MS_BF_VARIANT(64, 96),
+    MS_BF_VARIANT(128, 96),
+};
+#undef MS_BF_VARIANT
+
 int conv_bf_init() {
     static bool done = false;
     if (done) return 0;
-    MS_CHECK_CUDA(cudaFuncSetAttribute(conv_bf_kernel<64, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    MS_CHECK_CUDA(cudaFuncSetAttribute(conv_bf_kernel<64, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    MS_CHECK_CUDA(cudaFuncSetAttribute(conv_bf_kernel<96, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    MS_CHECK_CUDA(cudaFuncSetAttribute(conv_bf_kernel<96, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    MS_CHECK_CUDA(cudaFuncSetAttribute(conv_bf_kernel<128, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    MS_CHECK_CUDA(cudaFuncSetAttribute(conv_bf_kernel<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+    for (const BfVariant& v : BF_VARIANTS)
+        for (BfKernel k : v.k) MS_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     done = true;
     return 0;
 }
@@ -550,7 +613,8 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
     p.Hout = g.y.h; p.Wout = g.y.w; p.os = os; p.oy0 = oy0; p.ox0 = ox0;
     p.kch = Kpad > 32 ? 64 : 32;
     p.kblocks = Kpad / p.kch; p.cout = M; p.taps_total = taps_total;
-    p.wtile_bytes = 128u * (uint32_t)p.kch * 2u;
+    const int MT = bf_tile_rows(Mpad), CN = Mpad < 128 ? Mpad : 0;
+    p.wtile_bytes = (uint32_t)MT * (uint32_t)p.kch * 2u;
     p.fmt = xp.fmt; p.acc_scale = xp.fmt == 1 ? 1.f / xp.scale : 1.f;
     MS_REQUIRE(xp.fmt == 0 || xp.scale > 0.f, "conv_bf: fp16 planes need a positive scale");
     const uint32_t row_unit = (uint32_t)p.kch * 2u;                 // bytes of one pixel of a patch plane
@@ -577,23 +641,25 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
         }
         ++np;
     }
-    // ---- pixel tile TW x TH (N = TW * TH MMA columns, a multiple of 32, 64 <= N <= BF_MAX_N).  The tile shape decides
-    //      how many of the SMs work in the last wave: cost = waves x (N + fixed overhead in pixel units); ties go to the
-    //      taller tile (smaller halo).
-    const int mblocks = Mpad / 128;
+    // ---- pixel tile TW x TH (swap AB: N = TW * TH MMA columns, a multiple of 32, 64 <= N <= BF_MAX_N; pixel-major: N a
+    //      multiple of 64 -- whole m64 pixel blocks -- with at most 128 accumulator registers per thread).
+    //      The tile shape decides how many of the SMs work in the last wave: cost = waves x (MMA work of a tile + fixed
+    //      overhead, in units of 128-channel pixels); ties go to the taller tile (smaller halo).
+    const int mblocks = Mpad / MT;
+    const int max_n = CN ? std::min(256, 128 * 128 / CN) : BF_MAX_N;
     int N = 64, TW = 8;
     long best = -1; int best_th = 0;
     const int tws[3] = {8, 16, 32};
     for (int wi = 0; wi < 3; ++wi) {
         const int tw = tws[wi];
         if (tw * sx > 256) continue;
-        for (int th = 1; th * tw <= BF_MAX_N; ++th) {
+        for (int th = 1; th * tw <= max_n; ++th) {
             const int n = th * tw;
-            if (n < 64 || (n & 31)) continue;
+            if (n < 64 || (n & (CN ? 63 : 31)) || (CN && n == 192)) continue;
             if ((th + max_off) * sx > 256) continue;
             const long tiles = (long)g.y.n * cdiv(Wj, tw) * cdiv(Hj, th) * mblocks;
             // (halo rows are loaded, not multiplied: a quarter weight keeps 32 x 2 tiles for the cases that save a wave)
-            const long cost = cdiv((int)std::min<long>(tiles, 1 << 30), NUM_SMS) * (long)(n + 32 + max_off * tw / 4);
+            const long cost = cdiv((int)std::min<long>(tiles, 1 << 30), NUM_SMS) * (long)(n * MT / 128 + 32 + max_off * tw / 4);
             if (best < 0 || cost < best || (cost == best && th > best_th)) { best = cost; best_th = th; N = n; TW = tw; }
         }
     }
@@ -643,7 +709,7 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
     int ksplit = 1;
     if (part && tickets && (long)grid_tiles * mblocks <= NUM_SMS / 2 && units > 1) {
         ksplit = std::min(std::min(units, 8), std::max(1, NUM_SMS / (grid_tiles * mblocks)));
-        while (ksplit > 1 && (size_t)ksplit * grid_tiles * mblocks * N * 128 > conv_bf_part_floats()) --ksplit;
+        while (ksplit > 1 && (size_t)ksplit * grid_tiles * mblocks * N * MT > conv_bf_part_floats()) --ksplit;
         if ((size_t)grid_tiles * mblocks > conv_bf_ticket_words()) ksplit = 1;
     }
     p.ksplit = ksplit; p.part = part; p.tickets = tickets;
@@ -658,12 +724,13 @@ static int conv_bf_launch(const ConvGemm& g, const ActPlanes& xp, const void* wt
         if (bf_get_map(&mXl, xp.lo, 4, dims, strides, box, es, p.kch == 64 ? 128 : 64)) return -1;
     }
     // the epilogue stages the accumulators in the ring buffers
-    const size_t smem = std::max((size_t)NP * pslot + (size_t)NW * wslot, (size_t)N * BF_STAGE_LD * 4) + 1024;
+    const size_t smem = std::max((size_t)NP * pslot + (size_t)NW * wslot, (size_t)N * (CN ? CN + 4 : BF_STAGE_LD) * 4) + 1024;
     const dim3 grid(grid_tiles, mblocks, ksplit);
-    const bool bf = xp.fmt == 0;
-    if (N == 64) launch_k(bf ? conv_bf_kernel<64, 1> : conv_bf_kernel<64, 0>, grid, dim3(BF_THREADS), smem, st, *mXh, *mXl, p);
-    else if (N == 96) launch_k(bf ? conv_bf_kernel<96, 1> : conv_bf_kernel<96, 0>, grid, dim3(BF_THREADS), smem, st, *mXh, *mXl, p);
-    else launch_k(bf ? conv_bf_kernel<128, 1> : conv_bf_kernel<128, 0>, grid, dim3(BF_THREADS), smem, st, *mXh, *mXl, p);
+    const BfVariant* var = nullptr;
+    for (const BfVariant& v : BF_VARIANTS)
+        if (v.N == N && v.CN == CN) var = &v;
+    MS_REQUIRE(var != nullptr, "conv_bf: no kernel for this tile");
+    launch_k(var->k[xp.fmt == 0 ? 1 : 0], grid, dim3(BF_THREADS), smem, st, *mXh, *mXl, p);
     return check_launch("conv_bf");
 }
 

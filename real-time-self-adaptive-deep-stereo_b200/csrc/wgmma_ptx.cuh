@@ -30,6 +30,94 @@ template <int N, int BF, int TA, int TB>
 struct Wgmma;
 
 template <int TA, int TB>
+struct Wgmma<8, 1, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[4], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, %6, %7;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<8, 0, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[4], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, %6, %7;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<16, 1, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %10, %11;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<16, 0, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %10, %11;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<32, 1, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<32, 0, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<48, 1, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[24], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %26, %27;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
+struct Wgmma<48, 0, TA, TB> {
+    static __device__ __forceinline__ void mma(float (&d)[24], uint64_t a, uint64_t b) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %26, %27;\n\t}"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+            : "l"(a), "l"(b), "n"(TA), "n"(TB));
+    }
+};
+
+template <int TA, int TB>
 struct Wgmma<64, 1, TA, TB> {
     static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) {
         asm volatile(
