@@ -28,7 +28,11 @@ const char* ms_last_error(void);
  *   out[b,y,x,out_coff+i] = mean_c left[b,y,x,c] * RW[b,y,x+(-max_disp+i*stride),c]
  * `u` (optional, may be NULL) fuses MadNet._linear_warping (Nets/MadNet.py:400-436) of `right` by the
  * horizontal offsets u[b,y,x].  copy_left != 0 additionally writes left into out[...,0:C] (the tf.concat of
- * MadNet._stereo_cost_volume_correlation, Nets/MadNet.py:370-375) and the corr channels start at C. */
+ * MadNet._stereo_cost_volume_correlation, Nets/MadNet.py:370-375) and the corr channels start at C.
+ * Channels written, per pixel, whichever kernel the shape selects:
+ *   copy_left == 0: only [0, nd), nd = 2*max_disp/stride + 1; every other channel of `out` is left as it was.
+ *   copy_left != 0: [0, C) = left, [C, C+nd) = corr; channel C+nd is left as it was when u_chan != 0 (the caller has
+ *                   put u there); every channel from C+nd+u_chan up to out_cs is set to 0. */
 int ms_corr_fwd(const float* left, int left_cs, const float* right, int right_cs, const float* u, int u_cs,
                 float* out, int out_cs, int B, int h, int w, int C, int max_disp, int stride, int copy_left,
                 int u_chan, void* stream);

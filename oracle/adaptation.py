@@ -19,11 +19,13 @@ def softmax(x):
 class OracleAdapter:
     """One tf.train.MomentumOptimizer(lr, 0.9) shared by all train ops (one slot per variable)."""
 
-    def __init__(self, params, mode='MAD', lr=1e-4, mu=0.9, dtype=torch.float32, groups=None, loss='reprojection'):
+    def __init__(self, params, mode='MAD', lr=1e-4, mu=0.9, dtype=torch.float32, groups=None, loss='reprojection',
+                 radius_d=2, stride=1, warping=True, kink_signs=None):
         self.loss_kind = loss          # 'proxy': Stereo_Continual_Adaptation.py:75,112,133 (weights 0.01 / 0.1)
         assert mode in ('NONE', 'MAD', 'FULL')
         self.mode, self.lr, self.mu = mode, lr, mu
-        self.net = MadNetOracle(params, dtype=dtype, bulkhead=(mode == 'MAD'))
+        self.net = MadNetOracle(params, dtype=dtype, radius_d=radius_d, stride=stride, warping=warping,
+                                bulkhead=(mode == 'MAD'), kink_signs=kink_signs)
         self.groups = groups if groups is not None else mad_groups_full()
         self.momentum = {k: torch.zeros_like(v) for k, v in self.net.p.items()}
 

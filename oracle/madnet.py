@@ -23,15 +23,21 @@ LEVEL_FEAT = {6: 12, 5: 10, 4: 8, 3: 6, 2: 4}                            # level
 ALPHA = 0.2                                                              # MadNet.py:366-367
 
 
-def param_shapes(radius_d=2):
+def num_displacements(radius_d=2, stride=1):
+    """Channels of sharedLayers.correlation_tf: one per displacement in range(-d, d+1, stride) (sharedLayers.py:46)."""
+    return len(range(-radius_d, radius_d + 1, stride))
+
+
+def param_shapes(radius_d=2, stride=1):
     """OrderedDict TF-variable-name -> shape, in graph-construction order."""
     p = OrderedDict()
     for i in range(1, 13):
         s = 'model/gc-read-pyramid/conv%d' % i
         p[s + '/weights'] = (3, 3, PYRAMID_CH[i - 1], PYRAMID_CH[i])
         p[s + '/biases'] = (PYRAMID_CH[i],)
+    nd = num_displacements(radius_d, stride)
     for k in (6, 5, 4, 3, 2):
-        cin = PYRAMID_CH[LEVEL_FEAT[k]] + 2 * radius_d + 1 + (0 if k == 6 else 1)
+        cin = PYRAMID_CH[LEVEL_FEAT[k]] + nd + (0 if k == 6 else 1)
         for j, co in enumerate(EST_CH):
             s = 'model/G%d/fgc-volume-filtering-%d/disp-%d' % (k, k, j + 1)
             p[s + '/weights'] = (3, 3, cin, co)
@@ -46,7 +52,7 @@ def param_shapes(radius_d=2):
     return p
 
 
-def init_params(seed=42, bias_range=0.1, radius_d=2, conditioned=True):
+def init_params(seed=42, bias_range=0.1, radius_d=2, conditioned=True, stride=1):
     """Seeded xavier-uniform weights + small non-zero biases (SURVEY §8d).
 
     conditioned=True additionally rescales the draw so that a random net behaves like a trained one
@@ -57,7 +63,7 @@ def init_params(seed=42, bias_range=0.1, radius_d=2, conditioned=True):
     """
     rng = np.random.default_rng(seed)
     out = OrderedDict()
-    for name, shp in param_shapes(radius_d).items():
+    for name, shp in param_shapes(radius_d, stride).items():
         head = name.endswith('disp-6/weights') or name.endswith('context-7/weights')
         head_b = name.endswith('disp-6/biases') or name.endswith('context-7/biases')
         if len(shp) == 4:
@@ -80,41 +86,58 @@ def init_params(seed=42, bias_range=0.1, radius_d=2, conditioned=True):
 
 class MadNetOracle:
     def __init__(self, params, dtype=torch.float32, radius_d=2, stride=1, warping=True,
-                 context_net=True, bulkhead=False):
+                 context_net=True, bulkhead=False, kink_signs=None, kink_band=1e-4):
         self.p = OrderedDict((k, (v if torch.is_tensor(v) else torch.tensor(np.asarray(v))).to(dtype))
                              for k, v in params.items())
         self.dtype = dtype
         self.radius_d, self.stride = radius_d, stride
         self.warping, self.context_net, self.bulkhead = warping, context_net, bulkhead
         assert context_net, "context_net=False path is broken in the reference (MadNet.py:360)"
+        # kink_signs: {layer name: bool array, True where another implementation's output of that leaky-ReLU layer is
+        # > 0}.  Where this oracle's pre-activation lies within kink_band x the layer's largest |pre-activation| of zero,
+        # the slope follows that sign instead of its own; everywhere else the oracle is unchanged.  Two correct fp32
+        # computations can land on opposite sides of a kink for such an element, and then every gradient upstream of it
+        # differs by that element's share; with the other side's choice at those elements only, the float64 oracle
+        # measures the remaining arithmetic.  None (default): plain oracle.
+        self.kink_signs, self.kink_band = kink_signs, kink_band
+        self.kink_overrides = {}                      # layer name -> number of elements whose slope was taken over
 
     def requires_grad_(self, names=None):
         for k, v in self.p.items():
             v.requires_grad_(names is None or k in names)
 
-    def _conv(self, x, scope, stride=1, rate=1, alpha=ALPHA):
-        return T.conv2d(x, self.p[scope + '/weights'], self.p[scope + '/biases'],
-                        stride=stride, dilation=rate, alpha=alpha)
+    def _conv(self, x, scope, stride=1, rate=1, alpha=ALPHA, name=None):
+        if alpha is None or self.kink_signs is None or name not in self.kink_signs:
+            return T.conv2d(x, self.p[scope + '/weights'], self.p[scope + '/biases'],
+                            stride=stride, dilation=rate, alpha=alpha)
+        pre = T.conv2d(x, self.p[scope + '/weights'], self.p[scope + '/biases'], stride=stride, dilation=rate, alpha=None)
+        with torch.no_grad():
+            near = pre.abs() <= self.kink_band * pre.abs().max()
+            pos = torch.where(near, torch.as_tensor(np.asarray(self.kink_signs[name]), dtype=torch.bool), pre > 0)
+            self.kink_overrides[name] = int((near & (pos != (pre > 0))).sum())
+        return torch.where(pos, pre, pre * alpha)
 
     def pyramid(self, img, prefix, layers):
         x = img
         for i in range(1, 13):
-            x = self._conv(x, 'model/gc-read-pyramid/conv%d' % i, stride=2 if i % 2 == 1 else 1)
-            layers['%s/conv%d' % (prefix, i)] = x
+            name = '%s/conv%d' % (prefix, i)
+            x = self._conv(x, 'model/gc-read-pyramid/conv%d' % i, stride=2 if i % 2 == 1 else 1, name=name)
+            layers[name] = x
 
     def estimator(self, cost, u, k, layers):
         x = cost if u is None else torch.cat([cost, u], -1)
         for j in range(6):
+            name = 'fgc-volume-filtering-%d/disp%d' % (k, j + 1)
             x = self._conv(x, 'model/G%d/fgc-volume-filtering-%d/disp-%d' % (k, k, j + 1),
-                           alpha=ALPHA if j < 5 else None)
-            layers['fgc-volume-filtering-%d/disp%d' % (k, j + 1)] = x
+                           alpha=ALPHA if j < 5 else None, name=name)
+            layers[name] = x
         return x
 
     def context(self, feat, disp, layers):
         x = torch.cat([feat, disp], -1)
         for j in range(7):
             x = self._conv(x, 'model/context-%d' % (j + 1), rate=CTX_RATE[j],
-                           alpha=ALPHA if j < 6 else None)
+                           alpha=ALPHA if j < 6 else None, name='context%d' % (j + 1))
             layers['context%d' % (j + 1)] = x
         final = disp + x
         layers['final_disp'] = final

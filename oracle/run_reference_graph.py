@@ -50,16 +50,17 @@ def import_reference():
     return tfm, nets, loss_factory, preprocessing
 
 
-def build(model_name, mode, left, right, params):
-    """Stereo_Online_Adaptation.py:54-70 (network + full-resolution loss)."""
+def build(model_name, mode, left, right, params, net_args=None):
+    """Stereo_Online_Adaptation.py:54-70 (network + full-resolution loss).  `net_args` adds to / overrides the network
+    arguments (e.g. MADNet's radius_d, stride, warping; left unset, the network's own defaults apply)."""
     tf1_shim.reset_graph(params)
     tf, nets, loss_factory, preprocessing = import_reference()
     left_t = tf1_shim.TT(torch.as_tensor(left, dtype=torch.float32), 'input_reader/left')
     right_t = tf1_shim.TT(torch.as_tensor(right, dtype=torch.float32), 'input_reader/right')
     inputs = {'left': left_t, 'right': right_t, 'target': None}
     with tf.variable_scope('model'):
-        net_args = {'left_img': left_t, 'right_img': right_t, 'split_layers': [None], 'sequence': True,
-                    'train_portion': 'BEGIN', 'bulkhead': mode == 'MAD'}
+        net_args = dict({'left_img': left_t, 'right_img': right_t, 'split_layers': [None], 'sequence': True,
+                         'train_portion': 'BEGIN', 'bulkhead': mode == 'MAD'}, **(net_args or {}))
         stereo_net = nets.get_stereo_net(model_name, net_args)
         predictions = stereo_net.get_disparities()
     with tf.variable_scope('full_res_loss'):
@@ -192,9 +193,62 @@ def run_madnet_padded(out_path, h=100, w=200):
     print('wrote', out_path, '(%d arrays)' % len(out))
 
 
+# MADNet at non-default correlation settings: (radius_d, stride, warping) -> fixture name
+MADNET_VARIANTS = {(4, 2, False): 'reference_graph_madnet_r4s2_nowarp_64x128.npz',
+                   (2, 3, True): 'reference_graph_madnet_r2s3_warp_64x128.npz'}
+VARIANT_LAYERS = ('fgc-volume-filtering-6/disp1', 'fgc-volume-filtering-5/disp1', 'fgc-volume-filtering-4/disp3',
+                  'fgc-volume-filtering-2/disp1', 'fgc-volume-filtering-2/disp6', 'context5', 'final_disp')
+LEAKY_LAYERS = (['%s/conv%d' % (s, i) for s in ('left', 'right') for i in range(1, 13)] +
+                ['fgc-volume-filtering-%d/disp%d' % (k, j) for k in (6, 5, 4, 3, 2) for j in range(1, 6)] +
+                ['context%d' % j for j in range(1, 7)])
+VARIANT_GRADS = ('model/gc-read-pyramid/conv1/weights', 'model/gc-read-pyramid/conv12/weights',
+                 'model/G6/fgc-volume-filtering-6/disp-1/weights', 'model/G5/fgc-volume-filtering-5/disp-1/weights',
+                 'model/G3/fgc-volume-filtering-3/disp-1/weights', 'model/G2/fgc-volume-filtering-2/disp-1/weights',
+                 'model/G2/fgc-volume-filtering-2/disp-1/biases', 'model/context-4/weights')
+
+
+def run_madnet_variant(out_path, radius_d, stride, warping, h=64, w=128):
+    """The reference's Nets/MadNet.py with non-default radius_d / stride / warping: the estimators' input width follows
+    the correlation's displacement count (len(range(-d, d+1, s))).  Disparities, layers, the MAD and FULL losses and a
+    subsample of the FULL gradients.  `kink:<layer>` holds the sign (np.packbits of > 0) of every leaky-ReLU output of
+    the reference's fp32 run: where a pre-activation lies within rounding of zero, the reference's side of the kink decides
+    every gradient upstream of it, and the oracle can take the same side (MadNetOracle kink_signs)."""
+    from madstereo.synthetic import make_pair
+    from oracle.madnet import init_params
+    left, right, _ = make_pair(h, w, seed=3)
+    left = left.astype(np.float16).astype(np.float32); right = right.astype(np.float16).astype(np.float32)
+    params = {k: np.asarray(v) for k, v in init_params(seed=42, radius_d=radius_d, stride=stride).items()}
+    cfg = json.load(open(os.path.join(REF, 'block_config', 'MadNet_full.json')))
+    args = {'radius_d': radius_d, 'stride': stride, 'warping': warping}
+    out = {'left': left.astype(np.float16), 'right': right.astype(np.float16),
+           'net_args': np.array(json.dumps(args))}
+    tf, net, preds, full_loss, inputs, lf, pp = build('MADNet', 'MAD', left, right, params, args)
+    g = tf1_shim.graph()
+    out['variable_names'] = np.array([n for n, _ in g.created])
+    out['variable_shapes'] = np.array([json.dumps(list(s)) for _, s in g.created])
+    for i, d in enumerate(preds):
+        out['disp%d' % i] = d.numpy()
+    for k in VARIANT_LAYERS:
+        out['layer:' + k] = net[k].numpy()
+    for k in LEAKY_LAYERS:
+        out['kink:' + k] = np.packbits(net[k].numpy() > 0)
+    out['full_loss'] = np.float32(float(full_loss))
+    for k, (loss, _vars) in enumerate(mad_train_ops(tf, net, preds, inputs, lf, pp, cfg)):
+        out['mad%d_loss' % k] = np.float32(float(loss))
+    tf, net, preds, full_loss, inputs, lf, pp = build('MADNet', 'FULL', left, right, params, args)
+    gr = grads_of(full_loss, tf.get_collection(tf.GraphKeys.TRAINABLE_VARIABLES))
+    out['full_mode_loss'] = np.float32(float(full_loss))
+    for n in VARIANT_GRADS:
+        out['full_grad:' + n] = sub(gr[n])
+    np.savez_compressed(out_path, **out)
+    print('wrote', out_path, '(%d arrays)' % len(out))
+
+
 if __name__ == '__main__':
     torch.set_num_threads(1)
     gold = os.path.join(ROOT, 'tests', 'golden')
     run_madnet(os.path.join(gold, 'reference_graph_madnet_64x128.npz'))
     run_madnet_padded(os.path.join(gold, 'reference_graph_madnet_100x200.npz'))
     run_dispnet(os.path.join(gold, 'reference_graph_dispnet_64x128.npz'))
+    for (d, s, warp), name in MADNET_VARIANTS.items():
+        run_madnet_variant(os.path.join(gold, name), d, s, warp)

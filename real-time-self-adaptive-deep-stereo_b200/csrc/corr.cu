@@ -281,6 +281,7 @@ __global__ void __launch_bounds__(CORR_NT) corr_fwd2_kernel(CorrFwd p, int TW, i
             if (sub == 1) {
                 const float uu = p.u_chan ? o[5] : 0.f;                 // the u channel was written by the resize kernel
                 *reinterpret_cast<float4*>(o + 4) = make_float4(keep4, uu, 0.f, 0.f);
+                for (int c = coff + 8; c < p.ocs; ++c) orow[(size_t)x * p.ocs + c] = 0.f;
             }
         } else if (act && sub == 0 && p.copy_left) {
             for (int c = tail0; c < p.ocs; ++c) orow[(size_t)x * p.ocs + c] = 0.f;
@@ -419,6 +420,7 @@ __global__ void __launch_bounds__(CORR_NT) corr_fwd3_kernel(CorrFwd p, int TW, i
                     const float uu = p.u_chan ? o[5] : 0.f;
                     *reinterpret_cast<float4*>(o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
                     *reinterpret_cast<float4*>(o + 4) = make_float4(acc[4], uu, 0.f, 0.f);
+                    for (int c = coff + 8; c < p.ocs; ++c) orow[(size_t)x * p.ocs + c] = 0.f;
                 } else {
 #pragma unroll
                     for (int k = 0; k < AB; ++k)

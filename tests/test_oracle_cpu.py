@@ -2,6 +2,7 @@
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from oracle import tf1_ops as T
@@ -242,3 +243,46 @@ def test_oracle_batch_equals_single_frames():
                 assert d.shape[0] == 3 and _rel(d[b:b + 1].numpy(), r.numpy()) < 1e-5, (type(net).__name__, b, i)
             losses.append(float(T.reprojection_loss(d1[-1], torch.tensor(lb), torch.tensor(rb))))
         assert abs(loss - np.mean(losses)) <= 1e-6 * abs(loss), (type(net).__name__, loss, losses)
+
+
+VARIANT_GOLDENS = [(4, 2, False, 'reference_graph_madnet_r4s2_nowarp_64x128.npz'),
+                   (2, 3, True, 'reference_graph_madnet_r2s3_warp_64x128.npz')]
+
+
+@pytest.mark.parametrize('radius_d,stride,warping,name', VARIANT_GOLDENS)
+def test_oracle_matches_reference_graph_at_other_corr_settings(radius_d, stride, warping, name):
+    """The reference's Nets/MadNet.py with radius_d / stride / warping set (radius 4 stride 2 unwarped: 5 displacements
+    -4..4; radius 2 stride 3 warped: displacements -2, +1, where 2*radius_d is not a multiple of the stride).  The
+    estimators' input width follows the correlation's channel count, so the variable shapes pin param_shapes' stride
+    handling; disparities, layers, the MAD and FULL losses and the FULL gradients pin the oracle's forward and backward.
+    The gradients are taken with the float64 oracle on the reference's side of every leaky-ReLU kink that lies within rounding
+    of zero (the fixture's kink:<layer> signs; a handful of elements at most): there, the fp32 reference and the oracle
+    pick a side each, and a different pick moves every upstream gradient by far more than rounding."""
+    import json
+    g = np.load(os.path.join(os.path.dirname(__file__), 'golden', name))
+    assert json.loads(str(g['net_args'])) == {'radius_d': radius_d, 'stride': stride, 'warping': warping}
+    left = g['left'].astype(np.float32); right = g['right'].astype(np.float32)
+    shapes = param_shapes(radius_d, stride)
+    assert list(g['variable_names']) == list(shapes.keys())
+    assert [tuple(json.loads(s)) for s in g['variable_shapes']] == [tuple(v) for v in shapes.values()]
+    params = init_params(seed=42, radius_d=radius_d, stride=stride)
+    disps, layers = MadNetOracle(params, radius_d=radius_d, stride=stride, warping=warping).forward(left, right)
+    for i, d in enumerate(disps):
+        assert d.shape == g['disp%d' % i].shape
+        assert _rel(d.numpy(), g['disp%d' % i]) < 5e-5, i
+    for k in [k for k in g.files if k.startswith('layer:')]:
+        assert _rel(layers[k[6:]].numpy(), g[k]) < 5e-5, k
+    kw = dict(lr=1e-4, radius_d=radius_d, stride=stride, warping=warping)
+    for k in range(5):
+        out = OracleAdapter(params, mode='MAD', **kw).step(left, right, k)
+        assert abs(out['full_loss'] - float(g['full_loss'])) < 2e-6, k
+        assert abs(out['train_loss'] - float(g['mad%d_loss' % k])) < 2e-6, k
+    signs = {k[5:]: np.unpackbits(g[k], count=layers[k[5:]].numel()).reshape(layers[k[5:]].shape).astype(bool)
+             for k in g.files if k.startswith('kink:')}
+    assert len(signs) == 12 * 2 + 5 * 5 + 6
+    ad = OracleAdapter(params, mode='FULL', kink_signs=signs, dtype=torch.float64, **kw)
+    out = ad.step(left, right, 0)
+    assert sum(ad.net.kink_overrides.values()) <= 16, ad.net.kink_overrides
+    assert abs(out['train_loss'] - float(g['full_mode_loss'])) < 2e-6
+    for key in [x for x in g.files if x.startswith('full_grad:')]:
+        assert _rel(_sub(out['grads'][key.split(':', 1)[1]]), g[key]) < 2e-4, key
