@@ -68,30 +68,62 @@ int Engine::set_optimizer(int kind, float beta1, float beta2, float eps, float* 
     return 0;
 }
 
-void Engine::add_planes(Bump& A, const TView& v, int fmt) {
-    const bool sizing = A.base == nullptr;         // (sizing pass: pointers are null or null + a slice offset -- never dedupe)
-    if (!sizing && planes.count(v.p)) return;
-    ActPlanes pl;
-    pl.fmt = fmt;
-    pl.scale = fmt == 1 ? act_scale : 1.f;
-    pl.cs = (v.c + 7) / 8 * 8;
-    const size_t floats = (v.pixels() * pl.cs + 1) / 2;     // bf16 elements -> floats
-    pl.hi = A.alloc(floats);
-    pl.lo = A.alloc(floats);
-    if (!sizing) planes[v.p] = pl;
-}
-const ActPlanes* Engine::planes_of(const TView& v) const {
-    auto it = planes.find(v.p);
-    if (it == planes.end() || !it->second.hi || it->second.cs < v.c) return nullptr;
-    return &it->second;
-}
-int Engine::ensure_planes(const TView& v, cudaStream_t st) {
+int Engine::ensure_planes(const TView& v, const ActPlanes* pl, cudaStream_t st) {
     if (fresh.count(v.p)) return 0;
-    const ActPlanes* pl = planes_of(v);
-    MS_REQUIRE(pl != nullptr, "ensure_planes: tensor has no bf16 planes");
+    MS_REQUIRE(pl != nullptr, "ensure_planes: tensor has no 16-bit planes");
     if (split_planes(v, *pl, st)) return -1;
     fresh.insert(v.p);
     return 0;
+}
+// after a kernel wrote v: its planes are fresh if and only if the kernel wrote them too
+void Engine::planes_written(const TView& v, const ActPlanes* pl, bool written) {
+    if (written && pl) fresh.insert(v.p);
+    else fresh.erase(v.p);
+}
+
+// SAME padding of the layer's convolution from `in` to `out` (a transposed layer: of the stride-s conv that maps its
+// output back to its input); false if `out` is not the size that convolution produces
+static bool conv_pads(const ConvLayer& L, const TView& in, const TView& out, int& pt, int& pl) {
+    int oh, ow;
+    same_pad(in.h, L.kh, L.stride, L.dil, oh, pt);
+    same_pad(in.w, L.kw, L.stride, L.dil, ow, pl);
+    return oh == out.h && ow == out.w;
+}
+
+// Kernel arguments of a layer's three directions, shared by the planner and the dispatch so that both put the same
+// question to the kernels' predicates.  false: the views do not fit the layer.
+bool Engine::fwd_args(const ConvLayer& L, const TView& x, const TView& y, ConvGemm& p) const {
+    p = ConvGemm{};
+    p.x = x; p.y = y; p.kh = L.kh; p.kw = L.kw;
+    p.bias = Wt + L.b_off; p.alpha = L.alpha; p.mask_alpha = 1.f;
+    p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
+    int pt, pl;
+    const bool ok = L.transposed ? conv_pads(L, y, x, pt, pl) : conv_pads(L, x, y, pt, pl);
+    if (!L.transposed) { p.wmat = Wt + L.w_off; p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = L.dil; p.div = 1; }
+    // canonical W of a transposed layer is [tap][cout][cin]; the gather GEMM wants [tap][K=cin][N=cout] (transpose_taps)
+    else { p.wmat = wT; p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = L.stride; }
+    return ok && x.c == L.cin && y.c == L.cout;
+}
+// input gradient: the gather of dpre (a transposed layer: the stride-s conv of dpre with its canonical weights)
+bool Engine::dgrad_args(const ConvLayer& L, const TView& dpre, const TView& dx, ConvGemm& p) const {
+    p = ConvGemm{};
+    p.x = dpre; p.y = dx; p.wmat = Wt + L.w_off; p.kh = L.kh; p.kw = L.kw;
+    p.alpha = 1.f; p.mask_alpha = 1.f;
+    p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
+    int pt, pl;
+    const bool ok = L.transposed ? conv_pads(L, dpre, dx, pt, pl) : conv_pads(L, dx, dpre, pt, pl);
+    if (L.transposed) { p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1; }
+    else { p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -L.dil; p.div = L.stride; }
+    return ok && dpre.c == L.cout && dx.c == L.cin;
+}
+// weight gradient (a transposed layer: of the stride-s conv from its output-sized dpre to its input x; bias separately)
+bool Engine::wgrad_args(const ConvLayer& L, const TView& x, const TView& dpre, ConvWgrad& q) const {
+    q = ConvWgrad{};
+    q.x = L.transposed ? dpre : x; q.dy = L.transposed ? x : dpre;
+    q.dw = Gr + L.w_off; q.db = L.transposed ? nullptr : Gr + L.b_off;
+    q.kh = L.kh; q.kw = L.kw; q.stride = L.stride; q.dil = L.dil;
+    q.workspace = wg_ws; q.workspace_floats = wg_ws_floats;
+    return conv_pads(L, q.x, q.dy, q.pad_t, q.pad_l) && x.c == L.cin && dpre.c == L.cout;
 }
 
 void Engine::prof_reset() {
@@ -213,40 +245,127 @@ int Engine::finalize_groups(const int* group_of_layer, int ng) {
 // ---------------------------------------------------------------------------------------------
 // workspace layout
 // ---------------------------------------------------------------------------------------------
+void Engine::plan_views(int li, const TView& x, const TView& y, const TView& dpre, const TView& dx) {
+    plan[li] = ConvPlan{};
+    plan[li].x = x; plan[li].y = y; plan[li].dpre = dpre; plan[li].dx = dx;
+}
+
+// Every layer's kernels, in order of preference, from the views plan_views() recorded; then what they read: weight
+// tiles and prep jobs of BF forwards and dgrads, fp16 planes of BF forward inputs, bf16 planes of the output gradients
+// of BF dgrads and weight gradients, and the sizes of the weight-gradient workspace, its re-split scratch planes and
+// the transposed-weight scratch.
+void Engine::plan_convs(Bump& A, size_t& max_wg, size_t& max_wt) {
+    wg_xp_halfs = 0;
+    for (size_t li = 0; li < layers.size(); ++li) {
+        const ConvLayer& L = layers[li];
+        ConvPlan& P = plan[li];
+        ConvGemm f, d;
+        ConvWgrad q;
+        fwd_args(L, P.x, P.y, f);
+        wgrad_args(L, P.x, P.dpre, q);
+        if (conv_head_kind(f) == 1) P.fwd = ConvPlan::FWD_HEAD;
+        else if (conv_one_channel_supported(f)) P.fwd = ConvPlan::FWD_ONE_CHANNEL;
+        else if (!L.transposed && conv_stem_fwd_supported(f)) P.fwd = ConvPlan::FWD_STEM;
+        // the 16-channel full-resolution layers (conv2: 2 x 192 x 640 x 16) would fill one eighth of the swap-AB tile's
+        // accumulator rows; the shared-memory tiled direct kernel is bandwidth-shaped
+        else if (!L.transposed && conv_small_fwd_supported(f)) P.fwd = ConvPlan::FWD_SMALL;
+        else if (conv_bf_supported(f)) P.fwd = ConvPlan::FWD_BF;
+        else P.fwd = ConvPlan::FWD_GEMM;
+        // (an unaligned channel slice -- DispNet conv_redir's output gradient, channel 81 of gd_cat3 -- gets no planes:
+        //  its dgrad and weight gradient stay in fp32)
+        const bool dpre_planes = (reinterpret_cast<uintptr_t>(P.dpre.p) & 15) == 0;
+        P.dgrad = ConvPlan::DGRAD_GEMM;
+        if (P.dx.p && dgrad_args(L, P.dpre, P.dx, d)) {
+            if (conv_head_kind(d) == 2) P.dgrad = ConvPlan::DGRAD_HEAD;
+            else if (dpre_planes && conv_bf_supported(d)) P.dgrad = ConvPlan::DGRAD_BF;
+        }
+        // the image has no tensor-core weight gradient (MADNet conv1: conv_small_wgrad)
+        if (conv_stem_wgrad_supported(q)) P.wgrad = ConvPlan::WGRAD_STEM;
+        else if (P.x.p != img.p && dpre_planes && wgrad_bf_supported(q)) P.wgrad = ConvPlan::WGRAD_BF;
+        else if (conv_head_wgrad_supported(q)) P.wgrad = ConvPlan::WGRAD_HEAD;
+        else P.wgrad = ConvPlan::WGRAD_FP32;
+
+        const int taps = L.kh * L.kw;
+        size_t wg;
+        switch (P.wgrad) {
+        case ConvPlan::WGRAD_BF:    // wgrad_bf fits its split count to the workspace: 48 Mi floats bound the widest layers
+            wg = std::min<size_t>(wgrad_bf_workspace_floats(L.kh, L.kw, q.x.c, q.dy.c), (size_t)48 << 20);
+            wg_xp_halfs = std::max(wg_xp_halfs, P.x.pixels() * (size_t)((P.x.c + 7) / 8 * 8));
+            break;
+        case ConvPlan::WGRAD_STEM: wg = conv_stem_wgrad_workspace_floats(q); break;
+        case ConvPlan::WGRAD_HEAD: wg = conv_head_wgrad_workspace_floats(q); break;
+        default: wg = conv_wgrad_workspace_floats(taps, q.x.c, q.dy.c, q.dy.pixels());
+        }
+        if (L.transposed) wg = std::max(wg, (size_t)128 * L.cout);          // + bias_grad's partials (<= 128 blocks)
+        max_wg = std::max(max_wg, wg);
+        max_wt = std::max(max_wt, (size_t)taps * L.cin * L.cout);
+        if (P.fwd == ConvPlan::FWD_BF) planes[P.x.p] = ActPlanes{nullptr, nullptr, (P.x.c + 7) / 8 * 8, 1, 1.f};
+        if (P.dgrad == ConvPlan::DGRAD_BF || P.wgrad == ConvPlan::WGRAD_BF) planes[P.dpre.p] = ActPlanes{nullptr, nullptr, (P.dpre.c + 7) / 8 * 8, 0, 1.f};
+    }
+    // a tensor's planes cover the widest view any layer runs on (d_c2: conv2's output, conv_redir reads its left half)
+    std::map<const float*, size_t> pixels;
+    for (const ConvPlan& P : plan)
+        for (const TView* v : {&P.x, &P.y, &P.dpre, &P.dx})
+            if (planes.count(v->p)) pixels[v->p] = std::max(pixels[v->p], v->pixels());
+    for (auto& e : planes) {
+        ActPlanes& pl = e.second;
+        pl.scale = pl.fmt == 1 ? act_scale : 1.f;
+        pl.hi = A.alloc((pixels[e.first] * pl.cs + 1) / 2);           // 16-bit elements -> floats
+        pl.lo = A.alloc((pixels[e.first] * pl.cs + 1) / 2);
+    }
+    auto planes_of = [&](const TView& v) -> const ActPlanes* { auto it = planes.find(v.p); return it == planes.end() ? nullptr : &it->second; };
+    for (ConvPlan& P : plan) { P.xp = planes_of(P.x); P.yp = planes_of(P.y); P.dp = planes_of(P.dpre); P.dxp = planes_of(P.dx); }
+    // split 16-bit weight tiles of the BF directions (forward: fp16, dgrad: bf16), with their prep jobs grouped by MAD
+    // module so that an update refreshes exactly the tiles of the weights it moved
+    bf_jobs.clear(); bf_job_begin.assign(n_groups + 1, 0); bf_job_end.assign(n_groups + 1, 0);
+    bf_max_total = 0;
+    for (int gidx = 0; gidx <= n_groups; ++gidx) {
+        bf_job_begin[gidx] = (int)bf_jobs.size();
+        for (size_t li = 0; li < layers.size(); ++li) {
+            const ConvLayer& L = layers[li];
+            ConvPlan& P = plan[li];
+            if ((L.group < 0 ? n_groups : L.group) != gidx) continue;
+            for (int dir = 0; dir < 2; ++dir) {
+                if (dir == 0 ? P.fwd != ConvPlan::FWD_BF : P.dgrad != ConvPlan::DGRAD_BF) continue;
+                // forward: M = cout, K = cin; dgrad: M = cin, K = cout.  Canonical W is [tap][cin][cout] ([tap][cout][cin]
+                // for a transposed layer)
+                const int M = dir == 0 ? L.cout : L.cin, K = dir == 0 ? L.cin : L.cout;
+                int Mpad, Kpad; conv_bf_weight_dims(M, K, Mpad, Kpad);
+                const size_t halfs = conv_bf_weight_halfs(L.kh * L.kw, M, K);
+                P.tiles[dir] = A.alloc((halfs + 1) / 2);
+                bf_jobs.push_back(BfPrepJob{Wt ? Wt + L.w_off : nullptr, P.tiles[dir], L.kh * L.kw, M, K, Mpad, Kpad,
+                                            (dir == 0) != (L.transposed != 0), dir == 0 ? 1 : 0});
+                bf_max_total = std::max(bf_max_total, halfs);
+            }
+        }
+        bf_job_end[gidx] = (int)bf_jobs.size();
+    }
+}
+
 size_t Engine::layout(float* base) {
-    Bump A{base, 0};
+    // the sizing pass lays out against a stand-in base with the workspace's 256-byte alignment (never dereferenced), so
+    // that both passes plan from the same views
+    Bump A{base ? base : reinterpret_cast<float*>(uintptr_t{256}), 0};
     auto alloc = [&](size_t n) -> float* { return A.alloc(n); };
     auto tens = [&](int n, int h, int w, int c, int cs = 0) { return A.tens(n, h, w, c, cs); };
     tensors.clear();
     planes.clear(); fresh.clear();
+    plan.assign(layers.size(), ConvPlan{});
     char nm[128];
     const int nd = (2 * radius_d) / corr_stride + 1;
     TView raw_l = tens(B, H, W, 3), raw_r = tens(B, H, W, 3);
     tensors["raw_left"] = raw_l; tensors["raw_right"] = raw_r;
     img = tens(2 * B, Hp, Wp, 3, 4);
     tensors["img"] = img;
-    if (net == 1) add_planes(A, img, 1);           // DispNet's 7x7 stem runs on the tensor cores
-    size_t max_wg = 0, max_wt = 0;
-    auto track = [&](const ConvLayer& L, size_t pixels) {
-        max_wg = std::max(max_wg, conv_wgrad_workspace_floats(L.kh * L.kw, L.cin, L.cout, pixels));
-        max_wt = std::max(max_wt, (size_t)L.kh * L.kw * L.cin * L.cout);
-        if (L.cout == 1) max_wg = std::max(max_wg, (size_t)2 * NUM_SMS * ((size_t)L.kh * L.kw * L.cin + 1));    // conv_head_wgrad partials
-        if (!L.transposed && L.cin >= 3 && L.cout >= 16) {
-            max_wg = std::max(max_wg, std::min<size_t>(wgrad_bf_workspace_floats(L.kh, L.kw, L.cin, L.cout), (size_t)48 << 20));
-            wg_xp_halfs = std::max(wg_xp_halfs, pixels * L.stride * L.stride * (size_t)((L.cin + 7) / 8 * 8));
-        }
-    };
-    wg_xp_halfs = 0;
     if (net == 1) {
-        layout_dispnet(A, max_wg, max_wt);
+        layout_dispnet(A);
     } else {
     int h = Hp, w = Wp;
     for (int i = 1; i <= 12; ++i) {
         if (i % 2) { h = (h + 1) / 2; w = (w + 1) / 2; }
         pyr[i] = tens(2 * B, h, w, PYR_CH[i]);
         g_pyr[i] = tens(2 * B, h, w, PYR_CH[i]);
-        add_planes(A, pyr[i], 1); add_planes(A, g_pyr[i], 0);
-        track(layers[i - 1], (size_t)2 * B * h * w);
+        plan_views(i - 1, i > 1 ? pyr[i - 1] : img, pyr[i], g_pyr[i], i > 1 ? g_pyr[i - 1] : TView{});
         snprintf(nm, sizeof nm, "left/conv%d", i); tensors[nm] = batch(pyr[i], 0, B);
         snprintf(nm, sizeof nm, "right/conv%d", i); tensors[nm] = batch(pyr[i], B, B);
         snprintf(nm, sizeof nm, "grad/left/conv%d", i); tensors[nm] = batch(g_pyr[i], 0, B);
@@ -255,20 +374,17 @@ size_t Engine::layout(float* base) {
     ctxin = tens(B, pyr[4].h, pyr[4].w, PYR_CH[4] + 1, pad4(PYR_CH[4] + 1));
     g_ctxin = tens(B, pyr[4].h, pyr[4].w, PYR_CH[4] + 1, pad4(PYR_CH[4] + 1));
     tensors["ctxin"] = ctxin; tensors["grad/ctxin"] = g_ctxin;
-    add_planes(A, ctxin, 1);
     for (int k = 6; k >= 2; --k) {
         const int f = feat_of(k), C = PYR_CH[f];
         const int hh = pyr[f].h, ww = pyr[f].w;
         const int ct = C + nd + (k < 6 ? 1 : 0);
         cost[k] = tens(B, hh, ww, ct, pad4(ct));
         g_cost[k] = tens(B, hh, ww, ct, pad4(ct));
-        add_planes(A, cost[k], 1);
         snprintf(nm, sizeof nm, "cost%d", k); tensors[nm] = cost[k];
         snprintf(nm, sizeof nm, "grad/cost%d", k); tensors[nm] = g_cost[k];
         for (int j = 1; j <= 5; ++j) {
             est[k][j] = tens(B, hh, ww, EST_CH[j - 1]);
             g_est[k][j] = tens(B, hh, ww, EST_CH[j - 1]);
-            add_planes(A, est[k][j], 1); add_planes(A, g_est[k][j], 0);
             snprintf(nm, sizeof nm, "fgc-volume-filtering-%d/disp%d", k, j); tensors[nm] = est[k][j];
             snprintf(nm, sizeof nm, "grad/fgc-volume-filtering-%d/disp%d", k, j); tensors[nm] = g_est[k][j];
         }
@@ -279,19 +395,22 @@ size_t Engine::layout(float* base) {
         snprintf(nm, sizeof nm, "fgc-volume-filtering-%d/disp6", k); tensors[nm] = V[k];
         snprintf(nm, sizeof nm, "grad/fgc-volume-filtering-%d/disp6", k); tensors[nm] = g_V[k];
         snprintf(nm, sizeof nm, "grad/u%d", k); tensors[nm] = g_u[k];
-        for (int j = 1; j <= 6; ++j) track(layers[est_layer(k, j)], (size_t)B * hh * ww);
+        for (int j = 1; j <= 6; ++j)
+            plan_views(est_layer(k, j), j > 1 ? est[k][j - 1] : cost[k], j < 6 ? est[k][j] : V[k], j < 6 ? g_est[k][j] : g_V[k],
+                       j > 1 ? g_est[k][j - 1] : g_cost[k]);
     }
     for (int j = 1; j <= 6; ++j) {
         ctx[j] = tens(B, pyr[4].h, pyr[4].w, CTX_CH[j - 1]);
         g_ctx[j] = tens(B, pyr[4].h, pyr[4].w, CTX_CH[j - 1]);
-        add_planes(A, ctx[j], 1); add_planes(A, g_ctx[j], 0);
         snprintf(nm, sizeof nm, "context%d", j); tensors[nm] = ctx[j];
         snprintf(nm, sizeof nm, "grad/context%d", j); tensors[nm] = g_ctx[j];
     }
-    for (int j = 1; j <= 7; ++j) track(layers[ctx_layer(j)], (size_t)B * pyr[4].h * pyr[4].w);
     final_ = tens(B, pyr[4].h, pyr[4].w, 1);
     g_final = tens(B, pyr[4].h, pyr[4].w, 1);
     tensors["final_disp"] = final_; tensors["grad/final_disp"] = g_final;
+    for (int j = 1; j <= 7; ++j)
+        plan_views(ctx_layer(j), j > 1 ? ctx[j - 1] : ctxin, j < 7 ? ctx[j] : final_, j < 7 ? g_ctx[j] : g_final,
+                   j > 1 ? g_ctx[j - 1] : g_ctxin);
     }   // net == 0
     n_disp = net == 1 ? 7 : 6;
     for (int i = 0; i < n_disp; ++i) {
@@ -301,60 +420,10 @@ size_t Engine::layout(float* base) {
     tensors["rescaled_prediction"] = disp[n_disp - 1];
     g_disp = tens(B, H, W, 1);
     tensors["grad/disp"] = g_disp;
+    size_t max_wg = 0, max_wt = 0;
+    plan_convs(A, max_wg, max_wt);
     wT_floats = max_wt; wT = alloc(max_wt);
     wg_ws_floats = max_wg; wg_ws = alloc(max_wg);
-    // split 16-bit weight tiles per layer and orientation (forward: fp16, dgrad: bf16) + their batched prep job table
-    bfw[0].assign(layers.size(), BfW{nullptr, false});
-    bfw[1].assign(layers.size(), BfW{nullptr, false});
-    bf_jobs.clear(); bf_job_begin.assign(n_groups + 1, 0); bf_job_end.assign(n_groups + 1, 0);
-    bf_max_total = 0;
-    for (int gidx = 0; gidx <= n_groups; ++gidx) {
-        bf_job_begin[gidx] = (int)bf_jobs.size();
-        for (size_t li = 0; li < layers.size(); ++li) {
-            const ConvLayer& L = layers[li];
-            const int lg = L.group < 0 ? n_groups : L.group;
-            // (MADNet's 3 -> 16 conv1 stays on its direct kernel; a 3-channel stem with a large filter -- DispNet conv1, 7x7 --
-            //  is 2.3 GMAC and goes to the tensor cores with its K block zero-padded)
-            const bool stem = L.cin >= 3 && L.cin < 8 && L.kh * L.kw >= 25 && L.cout >= 16;
-            if (lg != gidx || (L.cin < 8 && !stem) || L.cout < 8 || L.kh * L.kw > 49 || L.stride > 2) continue;
-            if (L.transposed) {
-                // conv2d_transpose forward = fractionally strided gather: M = cout, K = cin, canonical W is already
-                // [tap][cout][cin] = [tap][M][K]
-                int Mpad, Kpad; conv_bf_weight_dims(L.cout, L.cin, Mpad, Kpad);
-                const size_t halfs = conv_bf_weight_halfs(L.kh * L.kw, L.cout, L.cin);
-                BfW t; t.ok = true;
-                t.tiles = alloc((halfs + 1) / 2);
-                bfw[0][li] = t;
-                BfPrepJob j{base ? Wt + L.w_off : nullptr, t.tiles, L.kh * L.kw, L.cout, L.cin, Mpad, Kpad, 0, 1};
-                bf_jobs.push_back(j);
-                bf_max_total = std::max(bf_max_total, halfs);
-                // its input gradient = the stride-2 conv of dY with the same filter read as HWIO [.,.,cout,cin]:
-                // M = cin, K = cout, canonical W = [tap][K][M]; bf16 (gradient planes)
-                conv_bf_weight_dims(L.cin, L.cout, Mpad, Kpad);
-                const size_t halfs_d = conv_bf_weight_halfs(L.kh * L.kw, L.cin, L.cout);
-                BfW td; td.ok = true;
-                td.tiles = alloc((halfs_d + 1) / 2);
-                bfw[1][li] = td;
-                BfPrepJob jd{base ? Wt + L.w_off : nullptr, td.tiles, L.kh * L.kw, L.cin, L.cout, Mpad, Kpad, 1, 0};
-                bf_jobs.push_back(jd);
-                bf_max_total = std::max(bf_max_total, halfs_d);
-                continue;
-            }
-            for (int dir = 0; dir < 2; ++dir) {
-                if (dir == 1 && stem) continue;                  // no input gradient for the image
-                const int M = dir == 0 ? L.cout : L.cin, K = dir == 0 ? L.cin : L.cout;
-                int Mpad, Kpad; conv_bf_weight_dims(M, K, Mpad, Kpad);
-                const size_t halfs = conv_bf_weight_halfs(L.kh * L.kw, M, K);
-                BfW t; t.ok = true;
-                t.tiles = alloc((halfs + 1) / 2);
-                bfw[dir][li] = t;
-                BfPrepJob j{base ? Wt + L.w_off : nullptr, t.tiles, L.kh * L.kw, M, K, Mpad, Kpad, dir == 0 ? 1 : 0, dir == 0 ? 1 : 0};
-                bf_jobs.push_back(j);
-                bf_max_total = std::max(bf_max_total, halfs);
-            }
-        }
-        bf_job_end[gidx] = (int)bf_jobs.size();
-    }
     if (wg_xp_halfs) {
         wg_xp.hi = alloc((wg_xp_halfs + 1) / 2); wg_xp.lo = alloc((wg_xp_halfs + 1) / 2); wg_xp.fmt = 0;
     }
@@ -376,135 +445,90 @@ size_t Engine::layout(float* base) {
 // ---------------------------------------------------------------------------------------------
 int Engine::conv_fwd(const ConvLayer& L, const TView& x, const TView& y, const float* res, int res_cs,
                      cudaStream_t st) {
-    ConvGemm p{};
-    p.x = x; p.y = y; p.kh = L.kh; p.kw = L.kw;
-    p.bias = Wt + L.b_off;
-    p.alpha = L.alpha;
-    p.res = res; p.res_cs = res_cs;
-    p.mask = nullptr; p.mask_cs = 0; p.mask_alpha = 1.f; p.accumulate = 0;
-    p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
-    int oh, ow, pt, pl;
-    if (!L.transposed) {
-        same_pad(x.h, L.kh, L.stride, L.dil, oh, pt);
-        same_pad(x.w, L.kw, L.stride, L.dil, ow, pl);
-        MS_REQUIRE(oh == y.h && ow == y.w && x.c == L.cin && y.c == L.cout, "conv_fwd: shape mismatch");
-        p.wmat = Wt + L.w_off;
-        p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = L.dil; p.div = 1;
-    } else {
-        same_pad(y.h, L.kh, L.stride, 1, oh, pt);
-        same_pad(y.w, L.kw, L.stride, 1, ow, pl);
-        MS_REQUIRE(oh == x.h && ow == x.w && x.c == L.cin && y.c == L.cout, "conv_fwd(T): shape mismatch");
-        p.wmat = wT;
-        p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = L.stride;
-        const int li_t = (int)(&L - &layers[0]);
-        const bool bf_t = bfw[0][li_t].ok && conv_bf_supported(p) && planes_of(x);
-        // canonical W is [tap][cout][cin]; the gather GEMM wants [tap][K=cin][N=cout] (the tensor-core path has its own tiles)
-        if (!bf_t && transpose_taps(Wt + L.w_off, wT, L.kh * L.kw, L.cout, L.cin, st)) return -1;
-    }
     const int li = (int)(&L - &layers[0]);
+    const ConvPlan& P = plan[li];
+    ConvGemm p;
+    MS_REQUIRE(same_view(x, P.x) && same_view(y, P.y) && fwd_args(L, x, y, p), "conv_fwd: views differ from the layer's plan");
+    p.res = res; p.res_cs = res_cs;
+    if (L.transposed && P.fwd != ConvPlan::FWD_BF && transpose_taps(Wt + L.w_off, wT, L.kh * L.kw, L.cout, L.cin, st)) return -1;
     prof_begin(CAT_CONV_FWD, st, li);
     int rc;
-    const ActPlanes* xpl = (bfw[0][li].ok && conv_bf_supported(p)) ? planes_of(x) : nullptr;
-    if (conv_head_kind(p) == 1) {
-        fresh.erase(y.p);
-        rc = conv_head(p, st);
-    } else if (L.cin == 1 && L.cout == 1 && conv_one_channel_supported(p)) {
-        fresh.erase(y.p);
+    switch (P.fwd) {
+    case ConvPlan::FWD_HEAD: rc = conv_head(p, st); break;
+    case ConvPlan::FWD_ONE_CHANNEL:
         p.wmat = Wt + L.w_off;                       // [tap][1][1]: canonical weights serve either orientation
         rc = conv_one_channel(p, st);
-    } else if (!L.transposed && (p.wmat = Wt + L.w_off, conv_stem_fwd_supported(p))) {
-        // DispNet conv1: 3 real channels per 32-wide K block on the tensor-core path; the CUDA cores do it in a third of the time
-        const ActPlanes* ypl = planes_of(y);
-        rc = conv_stem_fwd(p, ypl, st);
-        if (ypl) fresh.insert(y.p); else fresh.erase(y.p);
-    } else if (!L.transposed && L.cout <= 16 && conv_small_fwd_supported(p)) {
-        // full-resolution 16-channel layers (conv2: 2 x 192 x 640 x 16): M = cout = 16 would waste 7/8 of the swap-AB
-        // tile's accumulator rows and epilogue threads on the split-16-bit path; the shared-memory tiled direct
-        // kernel is bandwidth-shaped
-        fresh.erase(y.p);
-        rc = conv_small_fwd(p, st);
-    } else if (xpl) {
-        if (ensure_planes(x, st)) return -1;
-        const ActPlanes* ypl = planes_of(y);
-        rc = conv_bf(p, *xpl, bfw[0][li].tiles, ypl, bf_part, bf_tickets, st);
-        if (ypl) fresh.insert(y.p);
-    } else {
-        fresh.erase(y.p);
-        rc = conv_gemm(p, st);
+        break;
+    case ConvPlan::FWD_STEM: rc = conv_stem_fwd(p, P.yp, st); break;
+    case ConvPlan::FWD_SMALL: rc = conv_small_fwd(p, st); break;
+    case ConvPlan::FWD_BF:
+        rc = ensure_planes(x, P.xp, st);
+        if (!rc) rc = conv_bf(p, *P.xp, P.tiles[0], P.yp, bf_part, bf_tickets, st);
+        break;
+    default: rc = conv_gemm(p, st);
     }
+    planes_written(y, P.yp, P.fwd == ConvPlan::FWD_STEM || P.fwd == ConvPlan::FWD_BF);
     prof_end(st);
     prof_note((double)y.pixels() * L.kh * L.kw * L.cin * L.cout / (L.transposed ? L.stride * L.stride : 1), 0);
     return rc;
 }
 
+// weight gradient of a planned layer on stream st
+int Engine::wgrad(const ConvLayer& L, const ConvPlan& P, const ConvWgrad& q, cudaStream_t st) {
+    switch (P.wgrad) {
+    case ConvPlan::WGRAD_BF: {
+        // bf16 copy of the forward input in scratch planes: a wgmma takes one 16-bit element type for both operands, so
+        // the fp16 forward planes cannot pair with the bf16 gradient planes
+        ActPlanes xb = wg_xp; xb.cs = (P.x.c + 7) / 8 * 8;
+        MS_REQUIRE(P.x.pixels() * (size_t)xb.cs <= wg_xp_halfs, "wgrad: scratch planes too small");
+        if (split_planes(P.x, xb, st)) return -1;
+        return L.transposed ? wgrad_bf(q, *P.dp, xb, st) : wgrad_bf(q, xb, *P.dp, st);
+    }
+    case ConvPlan::WGRAD_STEM: return conv_stem_wgrad(q, st);           // DispNet conv1
+    case ConvPlan::WGRAD_HEAD: return conv_head_wgrad(q, st);           // single-channel heads, up_predict
+    default: return conv_wgrad(q, st);
+    }
+}
+
 // x: forward input of the layer; dpre: grad wrt pre-activation output; dx: where to write grad wrt x
 int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, const TView* dx_mask,
                      float mask_alpha, int dx_acc, int want_wgrad, cudaStream_t st) {
-    int oh, ow, pt, pl;
+    const int li = (int)(&L - &layers[0]);
+    const ConvPlan& P = plan[li];
     MS_REQUIRE(!L.transposed, "conv_bwd: transposed layers use deconv_bwd");
-    same_pad(x.h, L.kh, L.stride, L.dil, oh, pt);
-    same_pad(x.w, L.kw, L.stride, L.dil, ow, pl);
-    MS_REQUIRE(oh == dpre.h && ow == dpre.w && x.c == L.cin && dpre.c == L.cout, "conv_bwd: shape mismatch");
+    ConvWgrad q;
+    ConvGemm p;
+    MS_REQUIRE(same_view(x, P.x) && same_view(dpre, P.dpre) && wgrad_args(L, x, dpre, q) &&
+               (!dx || (same_view(*dx, P.dx) && dgrad_args(L, dpre, *dx, p))), "conv_bwd: views differ from the layer's plan");
     if (net == 1) fresh.clear();    // DispNet's backward mutates gradient tensors in place between convs: always re-split
     if (want_wgrad) {
-        ConvWgrad q{};
-        q.x = x; q.dy = dpre; q.dw = Gr + L.w_off; q.db = Gr + L.b_off;
-        q.kh = L.kh; q.kw = L.kw; q.stride = L.stride; q.dil = L.dil; q.pad_t = pt; q.pad_l = pl;
-        q.workspace = wg_ws; q.workspace_floats = wg_ws_floats; q.accumulate = 0;
-        prof_begin(CAT_CONV_WGRAD, st, (int)(&L - &layers[0]));
-        int rc = 0;
-        const bool stem_w = conv_stem_wgrad_supported(q);
-        const ActPlanes* wxp = (!stem_w && wgrad_bf_supported(q)) ? planes_of(x) : nullptr;
-        const ActPlanes* wdp = wxp ? planes_of(dpre) : nullptr;
+        prof_begin(CAT_CONV_WGRAD, st, li);
         // the planes of dpre also feed the dgrad below: they are produced on `st` BEFORE the fork
-        if (wxp && wdp) rc = ensure_planes(dpre, st);
+        int rc = P.wgrad == ConvPlan::WGRAD_BF ? ensure_planes(dpre, P.dp, st) : 0;
         cudaStream_t ws = st;
         if (!rc) rc = fork_wgrad(st, &ws);
-        if (!rc && wxp && wdp) {
-            // bf16 copy of the forward activation in scratch planes: a wgmma takes one 16-bit element type for both
-            // operands, so the fp16 forward planes cannot pair with the bf16 gradient planes
-            ActPlanes xb = wg_xp; xb.cs = (x.c + 7) / 8 * 8;
-            MS_REQUIRE(xb.hi && x.pixels() * (size_t)xb.cs <= wg_xp_halfs, "conv_bwd: wgrad scratch planes too small");
-            rc = split_planes(x, xb, ws);
-            if (!rc) rc = wgrad_bf(q, xb, *wdp, ws);
-        } else if (!rc && stem_w) {
-            rc = conv_stem_wgrad(q, ws);                 // DispNet conv1
-        } else if (!rc && conv_head_wgrad_supported(q)) {
-            rc = conv_head_wgrad(q, ws);                 // single-channel disparity heads
-        } else if (!rc) {
-            rc = conv_wgrad(q, ws);
-        }
+        if (!rc) rc = wgrad(L, P, q, ws);
         prof_end(st);
         prof_note((double)dpre.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
     }
     if (dx) {
-        ConvGemm p{};
-        p.x = dpre; p.wmat = wT; p.bias = nullptr; p.y = *dx; p.kh = L.kh; p.kw = L.kw;
-        p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -L.dil; p.div = L.stride;
-        p.alpha = 1.f;
         p.mask = dx_mask ? dx_mask->p : nullptr; p.mask_cs = dx_mask ? dx_mask->cs : 0; p.mask_alpha = mask_alpha;
-        p.res = nullptr; p.res_cs = 0; p.accumulate = dx_acc;
-        p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
-        const int li = (int)(&L - &layers[0]);
+        p.accumulate = dx_acc;
         prof_begin(CAT_CONV_DGRAD, st, li);
         int rc;
-        const ActPlanes* xpl = (bfw[1][li].ok && conv_bf_supported(p)) ? planes_of(dpre) : nullptr;
-        if (L.cout == 1 && (p.wmat = Wt + L.w_off, conv_head_kind(p) == 2)) {
-            fresh.erase(dx->p);
-            rc = conv_head(p, st);          // [tap][cin][1] == [tap][1][cin]: the canonical weights serve directly
-        } else if (xpl) {
+        switch (P.dgrad) {
+        case ConvPlan::DGRAD_HEAD: rc = conv_head(p, st); break;    // [tap][cin][1] == [tap][1][cin]: canonical weights
+        case ConvPlan::DGRAD_BF:
+            rc = ensure_planes(dpre, P.dp, st);
+            if (!rc) rc = conv_bf(p, *P.dp, P.tiles[1], P.dxp, bf_part, bf_tickets, st);
+            break;
+        default:
             p.wmat = wT;
-            rc = ensure_planes(dpre, st);
-            const ActPlanes* ypl = planes_of(*dx);
-            if (!rc) rc = conv_bf(p, *xpl, bfw[1][li].tiles, ypl, bf_part, bf_tickets, st);
-            if (ypl) fresh.insert(dx->p);
-        } else {
-            p.wmat = wT;
-            fresh.erase(dx->p);
             rc = transpose_taps(Wt + L.w_off, wT, L.kh * L.kw, L.cin, L.cout, st);   // -> [tap][cout][cin]
             if (!rc) rc = conv_gemm(p, st);
         }
+        planes_written(*dx, P.dxp, P.dgrad == ConvPlan::DGRAD_BF);
         prof_end(st);
         prof_note((double)dpre.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
@@ -843,7 +867,7 @@ int Engine::update(int group, float lr, float mu, float gscale, cudaStream_t st)
     } else if (momentum_update(Wt + b, Gr + b, Mo + b, e - b, lr, mu, gscale, st)) {
         return -1;
     }
-    return prep_layers(group, st);      // refresh the tf32 hi/lo copies of exactly the weights that moved
+    return prep_layers(group, st);      // refresh the 16-bit weight tiles of exactly the weights that moved
 }
 
 // forward + losses + backward (+ update) as one sequence; replayed as a CUDA graph after the first call
@@ -877,7 +901,7 @@ int Engine::run(int mode, int group, int disp_mask, int with_update, float lr, f
     MS_REQUIRE(!(with_update == 2 && mode != 0 && opt_kind != 0),
                "run: the fused data-parallel exchange (with_update=2) applies momentum only; Adam is single-GPU");
     if (profiling == 1) return run_eager(mode, group, disp_mask, with_update, lr, mu, gscale, st);
-    if (weights_dirty) {                    // load / restore happened: refresh every tf32 copy outside the graph
+    if (weights_dirty) {                    // load / restore happened: refresh every weight tile outside the graph
         if (prep_layers(-1, st)) return -1;
         weights_dirty = false;
     }

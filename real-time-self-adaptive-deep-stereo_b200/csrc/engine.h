@@ -30,11 +30,27 @@ struct DpState {               // device-resident exchange state of one rank (IP
     unsigned int epoch, blocks_done, error, pad;
 };
 
-struct Bump {            // workspace bump allocator (sizes only when base == nullptr)
+// Which kernel runs each direction of a layer.  Engine::plan_convs() decides it once per layout from the views the
+// layer runs on, with the kernels' own *_supported / conv_head_kind predicates, and allocates exactly what the chosen
+// kernels read; conv_fwd / conv_bwd / deconv_bwd only switch on it.
+struct ConvPlan {
+    enum Fwd { FWD_HEAD, FWD_ONE_CHANNEL, FWD_STEM, FWD_SMALL, FWD_BF, FWD_GEMM } fwd;
+    enum Dgrad { DGRAD_HEAD, DGRAD_BF, DGRAD_GEMM } dgrad;
+    enum Wgrad { WGRAD_BF, WGRAD_STEM, WGRAD_HEAD, WGRAD_FP32 } wgrad;   // FP32: conv_wgrad, which picks its own kernel
+    TView x, y, dpre, dx;                  // forward input / output, output and input gradients (dx.p == nullptr: none)
+    void* tiles[2];                        // split 16-bit weight tiles of a BF forward (0) and a BF dgrad (1)
+    const ActPlanes *xp, *yp, *dp, *dxp;   // 16-bit planes of x, y, dpre, dx; nullptr where no chosen kernel reads them
+};
+
+struct Bump {            // workspace bump allocator
     float* base; size_t off;
-    float* alloc(size_t n) { float* p = base ? base + off : nullptr; off += (n + 63) / 64 * 64; return p; }
+    float* alloc(size_t n) { float* p = base + off; off += (n + 63) / 64 * 64; return p; }
     TView tens(int n, int h, int w, int c, int cs = 0) { cs = cs ? cs : c; return view(alloc((size_t)n * h * w * cs), n, h, w, c, cs); }
 };
+
+inline bool same_view(const TView& a, const TView& b) {
+    return a.p == b.p && a.n == b.n && a.h == b.h && a.w == b.w && a.c == b.c && a.cs == b.cs;
+}
 
 // byte offset of the right frame in the uint8 staging buffer: the left frame's n bytes rounded up to 4
 inline size_t u8_stage_right_offset(size_t n) { return (n + 3) & ~(size_t)3; }
@@ -56,7 +72,6 @@ struct Engine {
 
     // tensors (valid after bind)
     std::map<std::string, TView> tensors;
-    std::string last_plan_error;
 
     // ---- MADNet buffers
     TView img;                       // [2B,Hp,Wp,3] cs=4
@@ -90,19 +105,23 @@ struct Engine {
     int backward_impl(int mode, int group, cudaStream_t st);
     int run(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st);
     int run_eager(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st);
-    // ---- split-16-bit wgmma path (conv_bf.cu): every eligible conv / dgrad / weight gradient
-    std::map<const float*, ActPlanes> planes;      // bf16 hi/lo planes of tensors that feed convolutions (key: base pointer)
-    std::set<const float*> fresh;                  // planes already written by a conv_bf epilogue in the current pass
-    struct BfW { void* tiles; bool ok; };
-    std::vector<BfW> bfw[2];                       // prepared weights per layer and orientation (0 = forward, 1 = dgrad)
+    // ---- per-layer kernel plan (ConvPlan) and the split-16-bit wgmma path (conv_bf.cu, wgrad_bf.cu)
+    std::vector<ConvPlan> plan;                    // per layer, filled by layout()
+    void plan_views(int li, const TView& x, const TView& y, const TView& dpre, const TView& dx);
+    void plan_convs(Bump& A, size_t& max_wg, size_t& max_wt);
+    std::map<const float*, ActPlanes> planes;      // 16-bit hi/lo planes of the tensors BF kernels read (key: base pointer)
+    std::set<const float*> fresh;                  // planes already written by a conv epilogue in the current pass
     std::vector<BfPrepJob> bf_jobs; std::vector<int> bf_job_begin, bf_job_end;
     BfPrepJob* bf_jobs_dev; size_t bf_max_total;
     float* bf_part; unsigned int* bf_tickets;
-    void add_planes(Bump& A, const TView& v, int fmt);      // fmt 1 = forward activation (fp16 of x/16), 0 = gradient (bf16)
     ActPlanes wg_xp; size_t wg_xp_halfs;              // bf16 scratch planes: forward activations re-split for the weight gradient
     float act_scale;                                  // power-of-two scale of the fp16 forward planes (per network)
-    const ActPlanes* planes_of(const TView& v) const;
-    int ensure_planes(const TView& v, cudaStream_t st);
+    int ensure_planes(const TView& v, const ActPlanes* pl, cudaStream_t st);
+    void planes_written(const TView& v, const ActPlanes* pl, bool written);
+    bool fwd_args(const ConvLayer& L, const TView& x, const TView& y, ConvGemm& p) const;
+    bool dgrad_args(const ConvLayer& L, const TView& dpre, const TView& dx, ConvGemm& p) const;
+    bool wgrad_args(const ConvLayer& L, const TView& x, const TView& dpre, ConvWgrad& q) const;
+    int wgrad(const ConvLayer& L, const ConvPlan& P, const ConvWgrad& q, cudaStream_t st);
     // ---- data-parallel exchange over NVLink peer memory (csrc/dp.cu)
     int dp_rank, dp_world; bool dp_connected;
     float* dp_xbuf; DpState* dp_state; size_t dp_cap_floats;
@@ -147,13 +166,13 @@ struct Engine {
     TView d_c1, d_c2, d_cat3, d_enc[8], d_cat[5], d_pr[5], d_cc[5], d_pred;
     TView gd_c1, gd_c2, gd_cat3, gd_enc[8], gd_cat[5], gd_pr[5], gd_cc[5], gd_pred;
     int build_dispnet();
-    void layout_dispnet(Bump& A, size_t& max_wg, size_t& max_wt);
+    void layout_dispnet(Bump& A);
     int forward_dispnet(int disp_mask, cudaStream_t st);
     int backward_dispnet(cudaStream_t st);
     int deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, int dx_acc, cudaStream_t st);
 
     Engine();
-    size_t layout(float* base);      // returns floats needed; assigns views when base != nullptr
+    size_t layout(float* base);      // returns floats needed; base == nullptr: sizing only (the views are not usable)
     int build_madnet();
     int finalize_groups(const int* group_of_layer, int n_groups);
 

@@ -49,46 +49,26 @@ int Engine::build_dispnet() {
     return 0;
 }
 
-void Engine::layout_dispnet(Bump& A, size_t& max_wg, size_t& max_wt) {
-    auto track = [&](const ConvLayer& L, size_t pixels) {
-        max_wg = std::max(max_wg, conv_wgrad_workspace_floats(L.kh * L.kw, L.cin, L.cout, pixels));
-        max_wg = std::max(max_wg, conv_wgrad_workspace_floats(L.kh * L.kw, L.cout, L.cin, pixels));
-        max_wt = std::max(max_wt, (size_t)L.kh * L.kw * L.cin * L.cout);
-        if (L.cout == 1) max_wg = std::max(max_wg, (size_t)2 * NUM_SMS * ((size_t)L.kh * L.kw * L.cin + 1));    // conv_head_wgrad partials
-        if (L.kh == 7 && L.cin == 3 && L.cout == 64) max_wg = std::max(max_wg, (size_t)2 * NUM_SMS * (147 * 64 + 64));   // conv_stem_wgrad partials
-        if (!L.transposed && L.cin >= 3 && L.cout >= 16) {
-            max_wg = std::max(max_wg, std::min<size_t>(wgrad_bf_workspace_floats(L.kh, L.kw, L.cin, L.cout), (size_t)48 << 20));
-            wg_xp_halfs = std::max(wg_xp_halfs, pixels * L.stride * L.stride * (size_t)((L.cin + 7) / 8 * 8));
-        }
-        if (L.transposed && L.cin >= 16 && L.cout >= 8) {
-            // conv2d_transpose: its weight gradient is the wgrad of the stride-2 conv big map (cout) -> small map (cin);
-            // `pixels` counts the big map, the bf16 scratch copy is of the small one (the layer's forward input)
-            max_wg = std::max(max_wg, std::min<size_t>(wgrad_bf_workspace_floats(L.kh, L.kw, L.cout, L.cin), (size_t)48 << 20));
-            wg_xp_halfs = std::max(wg_xp_halfs, pixels / (L.stride * L.stride) * (size_t)((L.cin + 7) / 8 * 8));
-        }
-        if (L.stride == 1 && !L.transposed && L.cout <= 192)
-            max_wg = std::max(max_wg, pixels * L.cout + 64 * (size_t)L.kh * L.kw * L.cin * L.cout + 128 * (size_t)L.cout + 8192);
-    };
-    const int h2 = Hp / 2, w2 = Wp / 2, h4 = Hp / 4, w4 = Wp / 4;
+void Engine::layout_dispnet(Bump& A) {
+    const int h2 = Hp / 2, w2 = Wp / 2, h4 = Hp / 4, w4 = Wp / 4, nd = 2 * DN_MAXD + 1;
     d_c1 = A.tens(2 * B, h2, w2, 64); gd_c1 = A.tens(2 * B, h2, w2, 64);
     d_c2 = A.tens(2 * B, h4, w4, 128); gd_c2 = A.tens(2 * B, h4, w4, 128);
     d_cat3 = A.tens(B, h4, w4, 145, 148); gd_cat3 = A.tens(B, h4, w4, 145, 148);
-    add_planes(A, d_c1, 1); add_planes(A, d_c2, 1); add_planes(A, d_cat3, 1);
-    add_planes(A, gd_c1, 0); add_planes(A, gd_c2, 0); add_planes(A, gd_cat3, 0);
-    track(layers[0], (size_t)2 * B * h2 * w2); track(layers[1], (size_t)2 * B * h4 * w4); track(layers[2], (size_t)B * h4 * w4);
+    plan_views(0, img, d_c1, gd_c1, TView{});
+    plan_views(1, d_c1, d_c2, gd_c2, gd_c1);
+    plan_views(2, batch(d_c2, 0, B), slice(d_cat3, nd, 64), slice(gd_cat3, nd, 64), batch(gd_c2, 0, B));
     int hh = h4, ww = w4;
     for (int i = 0; i < 8; ++i) {
         const ConvLayer& L = layers[3 + i];
         if (L.stride == 2) { hh /= 2; ww /= 2; }
         d_enc[i] = A.tens(B, hh, ww, L.cout); gd_enc[i] = A.tens(B, hh, ww, L.cout);
-        add_planes(A, d_enc[i], 1); add_planes(A, gd_enc[i], 0);
-        track(L, (size_t)B * hh * ww);
+        plan_views(3 + i, i ? d_enc[i - 1] : d_cat3, d_enc[i], gd_enc[i], i ? gd_enc[i - 1] : gd_cat3);
         tensors[L.name] = d_enc[i]; tensors["grad/" + L.name] = gd_enc[i];
     }
     tensors["conv1a"] = batch(d_c1, 0, B); tensors["conv1b"] = batch(d_c1, B, B);
     tensors["conv2a"] = batch(d_c2, 0, B); tensors["conv2b"] = batch(d_c2, B, B);
-    tensors["corr"] = slice(d_cat3, 0, 2 * DN_MAXD + 1);
-    tensors["conv_redir"] = slice(d_cat3, 2 * DN_MAXD + 1, 64);
+    tensors["corr"] = slice(d_cat3, 0, nd);
+    tensors["conv_redir"] = slice(d_cat3, nd, 64);
     tensors["grad/conv1"] = gd_c1; tensors["grad/conv2"] = gd_c2; tensors["grad/cat3"] = gd_cat3;
     // decoder: bottom of up5 is conv6/1 at Hp/64
     int bh = Hp / 64, bw = Wp / 64;
@@ -98,10 +78,12 @@ void Engine::layout_dispnet(Bump& A, size_t& max_wg, size_t& max_wt) {
         d_pr[u] = A.tens(B, bh, bw, 1); gd_pr[u] = A.tens(B, bh, bw, 1);
         d_cat[u] = A.tens(B, 2 * bh, 2 * bw, ct, pad4i(ct)); gd_cat[u] = A.tens(B, 2 * bh, 2 * bw, ct, pad4i(ct));
         d_cc[u] = A.tens(B, 2 * bh, 2 * bw, S.cout); gd_cc[u] = A.tens(B, 2 * bh, 2 * bw, S.cout);
-        add_planes(A, d_cat[u], 1); add_planes(A, d_cc[u], 1); add_planes(A, gd_cc[u], 0);
-        // compact bf16 planes of the deconv output's gradient (a channel slice of gd_cat[u], keyed by the slice pointer)
-        add_planes(A, slice(gd_cat[u], S.skip, S.cout), 0);
-        for (int j = 0; j < 4; ++j) track(layers[up_layer(u, j)], (size_t)B * 4 * bh * bw);
+        const TView bottom = u ? d_cc[u - 1] : d_enc[7], gbottom = u ? gd_cc[u - 1] : gd_enc[7];
+        // (the deconv output's gradient is a channel slice of gd_cat[u]: its planes are compact, keyed by the slice)
+        plan_views(up_layer(u, 0), bottom, slice(d_cat[u], S.skip, S.cout), slice(gd_cat[u], S.skip, S.cout), gbottom);
+        plan_views(up_layer(u, 1), bottom, d_pr[u], gd_pr[u], gbottom);
+        plan_views(up_layer(u, 2), d_pr[u], slice(d_cat[u], S.skip + S.cout, 1), slice(gd_cat[u], S.skip + S.cout, 1), gd_pr[u]);
+        plan_views(up_layer(u, 3), d_cat[u], d_cc[u], gd_cc[u], gd_cat[u]);
         std::string n(S.name);
         tensors[n + "/predict"] = d_pr[u];
         tensors[n + "/deconv"] = slice(d_cat[u], S.skip, S.cout);
@@ -111,7 +93,7 @@ void Engine::layout_dispnet(Bump& A, size_t& max_wg, size_t& max_wt) {
         bh *= 2; bw *= 2;
     }
     d_pred = A.tens(B, h2, w2, 1); gd_pred = A.tens(B, h2, w2, 1);
-    track(layers[DN_PRED], (size_t)B * h2 * w2);
+    plan_views(DN_PRED, d_cc[4], d_pred, gd_pred, gd_cc[4]);
     tensors["prediction"] = d_pred;
 }
 
@@ -167,52 +149,28 @@ int Engine::forward_dispnet(int disp_mask, cudaStream_t st) {
 //   dW[kh,kw,cout,cin] = wgrad of the stride-2 conv that maps the big map (channels cout) to the small one (channels cin)
 //   dx                 = that stride-2 conv applied to dpre with the same (canonical) weights as HWIO [.,.,cout,cin]
 int Engine::deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, int dx_acc, cudaStream_t st) {
-    MS_REQUIRE(L.transposed && dpre.h == x.h * L.stride && dpre.w == x.w * L.stride, "deconv_bwd: shape mismatch");
-    int keff = L.kh, oh = x.h;
-    int total = std::max((oh - 1) * L.stride + keff - dpre.h, 0);
-    const int pt = total / 2;
-    total = std::max((x.w - 1) * L.stride + L.kw - dpre.w, 0);
-    const int pl = total / 2;
     const int li = (int)(&L - &layers[0]);
-    const ActPlanes* dpl = planes_of(dpre);       // bf16 planes of the big map's gradient
-    if (dpl) { fresh.erase(dpre.p); if (ensure_planes(dpre, st)) return -1; }
+    const ConvPlan& P = plan[li];
+    MS_REQUIRE(L.transposed, "deconv_bwd: not a transposed layer");
+    ConvWgrad q;
+    ConvGemm p;
+    MS_REQUIRE(same_view(x, P.x) && same_view(dpre, P.dpre) && wgrad_args(L, x, dpre, q) &&
+               (!dx || (same_view(*dx, P.dx) && dgrad_args(L, dpre, *dx, p))), "deconv_bwd: views differ from the layer's plan");
+    if (P.dp) { fresh.erase(dpre.p); if (ensure_planes(dpre, P.dp, st)) return -1; }     // bf16 planes of the big map's gradient
     {
-        ConvWgrad q{};
-        q.x = dpre; q.dy = x; q.dw = Gr + L.w_off; q.db = nullptr;
-        q.kh = L.kh; q.kw = L.kw; q.stride = L.stride; q.dil = 1; q.pad_t = pt; q.pad_l = pl;
-        q.workspace = wg_ws; q.workspace_floats = wg_ws_floats; q.accumulate = 0;
         prof_begin(CAT_CONV_WGRAD, st, li);
-        int rc;
-        if (dpl && wg_xp.hi && wgrad_bf_supported(q)) {
-            // "x" = dY planes, "dy" = a bf16 re-split of the layer's forward input (a wgmma takes one 16-bit element type)
-            ActPlanes xb = wg_xp; xb.cs = (x.c + 7) / 8 * 8;
-            MS_REQUIRE(x.pixels() * (size_t)xb.cs <= wg_xp_halfs, "deconv_bwd: wgrad scratch planes too small");
-            rc = split_planes(x, xb, st);
-            if (!rc) rc = wgrad_bf(q, *dpl, xb, st);
-        } else if (conv_head_wgrad_supported(q)) {
-            rc = conv_head_wgrad(q, st);                 // up_predict: 1 -> 1 channel
-        } else {
-            rc = conv_wgrad(q, st);
-        }
+        int rc = wgrad(L, P, q, st);
         if (!rc) rc = bias_grad(dpre, Gr + L.b_off, wg_ws, wg_ws_floats, st);
         prof_end(st);
         prof_note((double)x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
     }
     if (dx) {
-        ConvGemm p{};
-        p.x = dpre; p.wmat = Wt + L.w_off; p.bias = nullptr; p.y = *dx; p.kh = L.kh; p.kw = L.kw;
-        p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1;
-        p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = dx_acc;
-        p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
+        p.accumulate = dx_acc;
         prof_begin(CAT_CONV_DGRAD, st, li);
-        int rc;
-        if (dpl && bfw[1][li].ok && conv_bf_supported(p)) {
-            fresh.erase(dx->p);                         // (accumulating launches leave dx's own planes stale)
-            rc = conv_bf(p, *dpl, bfw[1][li].tiles, nullptr, bf_part, bf_tickets, st);
-        } else {
-            rc = conv_gemm(p, st);
-        }
+        // (an accumulating launch would leave dx's own planes stale: it writes none)
+        const int rc = P.dgrad == ConvPlan::DGRAD_BF ? conv_bf(p, *P.dp, P.tiles[1], nullptr, bf_part, bf_tickets, st) : conv_gemm(p, st);
+        planes_written(*dx, P.dxp, false);
         prof_end(st);
         prof_note((double)x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
@@ -229,8 +187,6 @@ int Engine::backward_dispnet(cudaStream_t st) {
     if (conv_bwd(layers[DN_PRED], d_cc[4], gd_pred, &gd_cc[4], nullptr, 1.f, 0, 1, st)) return -1;
 
     TView c2a = batch(d_c2, 0, B);
-    const TView skips[5] = {d_enc[5], d_enc[3], d_enc[1], c2a, batch(d_c1, 0, B)};
-    TView gskip[5] = {gd_enc[5], gd_enc[3], gd_enc[1], batch(gd_c2, 0, B), batch(gd_c1, 0, B)};
     for (int u = 4; u >= 0; --u) {
         const UpSpec& S = DN_UP[u];
         const TView bottom = u == 0 ? d_enc[7] : d_cc[u - 1];
@@ -246,7 +202,6 @@ int Engine::backward_dispnet(cudaStream_t st) {
         if (conv_bwd(layers[up_layer(u, 1)], bottom, gd_pr[u], &gbottom, nullptr, 1.f, 0, 1, st)) return -1;
         // deconv (transposed, leaky already applied): -> gbottom (accumulate)
         if (deconv_bwd(layers[up_layer(u, 0)], bottom, g_dec, &gbottom, 1, st)) return -1;
-        (void)skips;
     }
     // ---- encoder, top down.  gd_enc[7] = d(conv6/1 output) complete.
     // feature grads that also receive a skip-slice contribution: enc[5] (up5), enc[3] (up4), enc[1] (up3)
