@@ -192,11 +192,12 @@ struct ReprojLoss {
     const float* disp;                        // [B,H,W,1]
     float* loss;                              // device scalar out
     float* ddisp;                             // optional [B,H,W,1] gradient out (nullptr = forward only)
-    float* workspace;                         // >= loss_workspace_floats(B,H,W)
+    float* workspace;                         // >= loss_workspace_floats(B,H,W) (no ddisp: loss_value_workspace_floats)
     int B, H, W;
     float grad_scale;                         // multiplies the gradient (1 for a single rank)
 };
 size_t loss_workspace_floats(int B, int H, int W);
+size_t loss_value_workspace_floats(int B, int H, int W);
 int reproj_loss(const ReprojLoss& p, cudaStream_t st);
 int epe_bad3(const float* disp, const float* gt, int n, float* out2, float* workspace, cudaStream_t st);
 // masked mean-L1 against proxy disparities (loss_factory.get_proxy_loss('mean_l1')); workspace >= 2 * ceil(n/256) + 2 floats

@@ -38,12 +38,13 @@ Engine::Engine()
       wg_ws(nullptr), wg_ws_floats(0), rs_tmp(nullptr), rs_tmp_floats(0), loss_ws(nullptr), loss_ws_floats(0),
       scalars(nullptr), gt(nullptr), proxy(nullptr), loss_kind(0), proxy_w_full(0.01f), proxy_w_module(0.1f), profiling(0), prof_capturing(false), prof_event_overhead_ms(0.f) {
     prof_reset();
-    gemm_part = nullptr; weights_dirty = true;
+    splitk[0] = splitk[1] = SplitK{nullptr, nullptr, nullptr}; on_branch = 0; weights_dirty = true;
     gstream = nullptr; ev_in = nullptr; ev_out = nullptr;
     wstream = nullptr; ev_fork = nullptr; ev_join = nullptr; wstream_dirty = false;
+    bstream = nullptr; ev_bfork = nullptr; ev_bjoin = nullptr; loss_full_ws = nullptr;
     wg_xp.hi = wg_xp.lo = nullptr; wg_xp.cs = 0; wg_xp.fmt = 0; wg_xp.scale = 1.f; wg_xp_halfs = 0;
     act_scale = 0.f;
-    bf_jobs_dev = nullptr; bf_max_total = 0; bf_part = nullptr; bf_tickets = nullptr;
+    bf_jobs_dev = nullptr; bf_max_total = 0;
     dp_rank = 0; dp_world = 1; dp_connected = false; dp_xbuf = nullptr; dp_state = nullptr; dp_cap_floats = 0;
     opt_kind = 0; adam_b1 = adam_b2 = adam_eps = 0.f; adam_v = nullptr; adam_powers = nullptr;
 }
@@ -96,7 +97,7 @@ bool Engine::fwd_args(const ConvLayer& L, const TView& x, const TView& y, ConvGe
     p = ConvGemm{};
     p.x = x; p.y = y; p.kh = L.kh; p.kw = L.kw;
     p.bias = Wt + L.b_off; p.alpha = L.alpha; p.mask_alpha = 1.f;
-    p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
+    p.part = sk().gemm_part; p.part_floats = conv_gemm_part_floats();
     int pt, pl;
     const bool ok = L.transposed ? conv_pads(L, y, x, pt, pl) : conv_pads(L, x, y, pt, pl);
     if (!L.transposed) { p.wmat = Wt + L.w_off; p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = L.dil; p.div = 1; }
@@ -109,7 +110,7 @@ bool Engine::dgrad_args(const ConvLayer& L, const TView& dpre, const TView& dx, 
     p = ConvGemm{};
     p.x = dpre; p.y = dx; p.wmat = Wt + L.w_off; p.kh = L.kh; p.kw = L.kw;
     p.alpha = 1.f; p.mask_alpha = 1.f;
-    p.part = gemm_part; p.part_floats = conv_gemm_part_floats();
+    p.part = sk().gemm_part; p.part_floats = conv_gemm_part_floats();
     int pt, pl;
     const bool ok = L.transposed ? conv_pads(L, dpre, dx, pt, pl) : conv_pads(L, dx, dpre, pt, pl);
     if (L.transposed) { p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1; }
@@ -427,16 +428,30 @@ size_t Engine::layout(float* base) {
     if (wg_xp_halfs) {
         wg_xp.hi = alloc((wg_xp_halfs + 1) / 2); wg_xp.lo = alloc((wg_xp_halfs + 1) / 2); wg_xp.fmt = 0;
     }
-    bf_part = alloc(conv_bf_part_floats());
-    bf_tickets = reinterpret_cast<unsigned int*>(alloc(conv_bf_ticket_words()));
+    splitk[0].bf_part = alloc(conv_bf_part_floats());
+    splitk[0].bf_tickets = reinterpret_cast<unsigned int*>(alloc(conv_bf_ticket_words()));
     bf_jobs_dev = reinterpret_cast<BfPrepJob*>(alloc((bf_jobs.size() + 1) * sizeof(BfPrepJob) / sizeof(float) + 16));
-    gemm_part = alloc(conv_gemm_part_floats());
+    splitk[0].gemm_part = alloc(conv_gemm_part_floats());
     rs_tmp_floats = (size_t)B * H * Wp; rs_tmp = alloc(rs_tmp_floats);
     loss_ws_floats = loss_workspace_floats(B, H, W); loss_ws = alloc(loss_ws_floats);
     scalars = alloc(64);
     u8_stage = reinterpret_cast<unsigned char*>(alloc((2 * u8_stage_right_offset((size_t)B * H * W * 3)) / 4 + 64));
     gt = alloc((size_t)B * H * W);
     proxy = alloc((size_t)B * H * W);
+    // what a MAD train op on its branch (mad_branch) shares with the forward's tail: the split-K scratch of its dgrads
+    // and the loss workspace.  Its own copies; everything else it writes (g_*, Gr, Mo, wg_ws, wg_xp, rs_tmp, g_disp, the
+    // module's weights and tiles, scalars[1]) no later forward kernel touches, and the tail runs no conv on wT
+    splitk[1] = splitk[0];
+    loss_full_ws = nullptr;
+    if (net == 0 && n_groups > 0) {
+        splitk[1].bf_part = alloc(conv_bf_part_floats());
+        splitk[1].bf_tickets = reinterpret_cast<unsigned int*>(alloc(conv_bf_ticket_words()));
+        bool module_gemm = false;
+        for (size_t li = 0; li < layers.size(); ++li)
+            module_gemm |= layers[li].group >= 0 && plan[li].dx.p && plan[li].dgrad == ConvPlan::DGRAD_GEMM;
+        if (module_gemm) splitk[1].gemm_part = alloc(conv_gemm_part_floats());
+        loss_full_ws = alloc(loss_value_workspace_floats(B, H, W));
+    }
     return A.off;
 }
 
@@ -463,7 +478,7 @@ int Engine::conv_fwd(const ConvLayer& L, const TView& x, const TView& y, const f
     case ConvPlan::FWD_SMALL: rc = conv_small_fwd(p, st); break;
     case ConvPlan::FWD_BF:
         rc = ensure_planes(x, P.xp, st);
-        if (!rc) rc = conv_bf(p, *P.xp, P.tiles[0], P.yp, bf_part, bf_tickets, st);
+        if (!rc) rc = conv_bf(p, *P.xp, P.tiles[0], P.yp, sk().bf_part, sk().bf_tickets, st);
         break;
     default: rc = conv_gemm(p, st);
     }
@@ -521,7 +536,7 @@ int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, cons
         case ConvPlan::DGRAD_HEAD: rc = conv_head(p, st); break;    // [tap][cin][1] == [tap][1][cin]: canonical weights
         case ConvPlan::DGRAD_BF:
             rc = ensure_planes(dpre, P.dp, st);
-            if (!rc) rc = conv_bf(p, *P.dp, P.tiles[1], P.dxp, bf_part, bf_tickets, st);
+            if (!rc) rc = conv_bf(p, *P.dp, P.tiles[1], P.dxp, sk().bf_part, sk().bf_tickets, st);
             break;
         default:
             p.wmat = wT;
@@ -582,8 +597,14 @@ int Engine::prep_layers(int group, cudaStream_t st) {
     return bf_prep_weights(bf_jobs_dev + b, e - b, bf_max_total, st);
 }
 
-int Engine::forward(int disp_mask, cudaStream_t st) {
+int Engine::forward(int disp_mask, cudaStream_t st, int fork_group, cudaStream_t branch) {
     MS_REQUIRE(bound, "engine not bound");
+    MS_REQUIRE(!branch || (net == 0 && fork_group >= 0 && fork_group <= 4), "forward: bad branch point");
+    auto fork = [&]() -> int {
+        MS_CHECK_CUDA(cudaEventRecord(ev_bfork, st));
+        MS_CHECK_CUDA(cudaStreamWaitEvent(branch, ev_bfork, 0));
+        return 0;
+    };
     fresh.clear();
     const int nd = (2 * radius_d) / corr_stride + 1;
     {
@@ -635,6 +656,7 @@ int Engine::forward(int disp_mask, cudaStream_t st) {
             if (conv_fwd(layers[est_layer(k, j)], xin, y, nullptr, 0, st)) return -1;
             xin = y;
         }
+        if (branch && fork_group == 6 - k && fork()) return -1;
     }
     {
         TView xin = ctxin;
@@ -643,14 +665,16 @@ int Engine::forward(int disp_mask, cudaStream_t st) {
             if (conv_fwd(layers[ctx_layer(j)], xin, y, j == 7 ? V[2].p : nullptr, V[2].cs, st)) return -1;
             xin = y;
         }
+        if (branch && fork_group == 4 && fork()) return -1;
     }
     for (int i = 0; i < 6; ++i) {
         if (!(disp_mask & (1 << i))) continue;
         const TView& src = (i < 4) ? V[6 - i] : final_;
+        cudaStream_t s = branch && i == fork_group ? branch : st;
         if (i < 5) {
-            if (resize_bilinear(src.p, src.cs, B, src.h, src.w, disp[i].p, 1, Hp, Wp, H, W, -20.f, 1, 1.f, 0, st)) return -1;
+            if (resize_bilinear(src.p, src.cs, B, src.h, src.w, disp[i].p, 1, Hp, Wp, H, W, -20.f, 1, 1.f, 0, s)) return -1;
         } else {
-            if (resize_bilinear(src.p, src.cs, B, src.h, src.w, disp[i].p, 1, Hp, Wp, H, W, 1.f, 0, -20.f, 1, st)) return -1;
+            if (resize_bilinear(src.p, src.cs, B, src.h, src.w, disp[i].p, 1, Hp, Wp, H, W, 1.f, 0, -20.f, 1, s)) return -1;
         }
     }
     return 0;
@@ -658,12 +682,14 @@ int Engine::forward(int disp_mask, cudaStream_t st) {
 
 int Engine::loss(int which, int with_grad, int slot, float grad_scale, cudaStream_t st) {
     MS_REQUIRE(bound && which >= 0 && which < n_disp && slot >= 0 && slot < 2, "loss: bad arguments");
+    // the full-resolution loss of a MAD step runs beside the module's loss (mad_branch): a workspace of its own
+    float* ws = slot == 0 && !with_grad && loss_full_ws ? loss_full_ws : loss_ws;
     if (loss_kind == 1) {
         // Stereo_Continual_Adaptation.py:75 (full-resolution loss, weight 0.01; also the FULL train op :133) and :112
         // (module losses, weight 0.1)
         const float wgt = slot == 0 ? proxy_w_full : proxy_w_module;
         prof_begin(CAT_LOSS, st);
-        int rc = proxy_loss(disp[which].p, proxy, B * H * W, wgt, grad_scale, scalars + slot, with_grad ? g_disp.p : nullptr, loss_ws, st);
+        int rc = proxy_loss(disp[which].p, proxy, B * H * W, wgt, grad_scale, scalars + slot, with_grad ? g_disp.p : nullptr, ws, st);
         prof_end(st);
         return rc;
     }
@@ -671,7 +697,7 @@ int Engine::loss(int which, int with_grad, int slot, float grad_scale, cudaStrea
     p.left = tensors["raw_left"].p; p.right = tensors["raw_right"].p;
     p.disp = disp[which].p; p.loss = scalars + slot;
     p.ddisp = with_grad ? g_disp.p : nullptr;
-    p.workspace = loss_ws; p.B = B; p.H = H; p.W = W; p.grad_scale = grad_scale;
+    p.workspace = ws; p.B = B; p.H = H; p.W = W; p.grad_scale = grad_scale;
     prof_begin(CAT_LOSS, st);
     int rc = reproj_loss(p, st);
     prof_end(st);
@@ -870,6 +896,16 @@ int Engine::update(int group, float lr, float mu, float gscale, cudaStream_t st)
     return prep_layers(group, st);      // refresh the 16-bit weight tiles of exactly the weights that moved
 }
 
+// Only while a step graph is captured without instrumentation (run() calls run_eager directly only to profile), and only
+// when no layer of the module runs after its disparity head: its update must not move weights the forward's tail reads.
+bool Engine::mad_branch(int mode, int group) const {
+    if (mode != 1 || profiling || net != 0 || group < 0 || group > 4) return false;
+    const int head = group < 4 ? est_layer(6 - group, 6) : ctx_layer(7);     // layers are indexed in forward order
+    for (size_t li = 0; li < layers.size(); ++li)
+        if (layers[li].group == group && (int)li > head) return false;
+    return true;
+}
+
 // forward + losses + backward (+ update) as one sequence; replayed as a CUDA graph after the first call
 int Engine::run_eager(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale,
                       cudaStream_t st) {
@@ -878,14 +914,38 @@ int Engine::run_eager(int mode, int group, int disp_mask, int with_update, float
     if (mode == 1) mask |= 1 << group;
     // NVTX ranges (SURVEY section 5: tracing): visible in nsys / ncu timelines, free when no tool is attached
     struct Range { explicit Range(const char* n) { nvtxRangePushA(n); } ~Range() { nvtxRangePop(); } };
-    { Range r("madstereo/forward"); if (forward(mask, st)) return -1; }
+    const bool branch = mad_branch(mode, group);
+    if (branch && !bstream) {
+        MS_CHECK_CUDA(cudaStreamCreateWithFlags(&bstream, cudaStreamNonBlocking));
+        MS_CHECK_CUDA(cudaEventCreateWithFlags(&ev_bfork, cudaEventDisableTiming));
+        MS_CHECK_CUDA(cudaEventCreateWithFlags(&ev_bjoin, cudaEventDisableTiming));
+    }
+    cudaStream_t bs = branch ? bstream : st;     // the train op's stream
+    { Range r("madstereo/forward"); if (forward(mask, st, branch ? group : -1, branch ? bstream : nullptr)) return -1; }
     { Range r("madstereo/loss_full"); if (loss(full, mode == 2, 0, 1.f, st)) return -1; }
     if (mode == 1) {
-        { Range r("madstereo/loss_module"); if (loss(group, 1, 1, 1.f, st)) return -1; }
-        { Range r("madstereo/backward_mad"); if (backward(1, group, st)) return -1; }
-        Range r("madstereo/update");
-        if (with_update == 1 && update(group, lr, mu, gscale, st)) return -1;
-        if (with_update == 2 && dp_update(group, lr, mu, st)) return -1;       // all-reduce over peer memory + update
+        auto train_op = [&]() -> int {
+            { Range r("madstereo/loss_module"); if (loss(group, 1, 1, 1.f, bs)) return -1; }
+            { Range r("madstereo/backward_mad"); if (backward(1, group, bs)) return -1; }
+            Range r("madstereo/update");
+            return with_update == 1 ? update(group, lr, mu, gscale, bs) : 0;
+        };
+        // The branch's kernels launch without PDL: their CTAs would otherwise become resident early and wait in
+        // griddepcontrol.wait, holding SM resources that the forward's tail and the weight gradients beside them could
+        // use (tools/step_phases.py: faster for every module, most for module 4, whose dgrad chain is the longest)
+        const bool pdl = pdl_enabled();
+        on_branch = branch ? 1 : 0;
+        if (branch) pdl_set_suppressed(true);
+        const int rc = train_op();
+        pdl_set_suppressed(!pdl);
+        on_branch = 0;
+        if (branch) {       // always joined: a captured side branch must be joined before the capture ends
+            MS_CHECK_CUDA(cudaEventRecord(ev_bjoin, bs));
+            MS_CHECK_CUDA(cudaStreamWaitEvent(st, ev_bjoin, 0));
+        }
+        if (rc) return rc;
+        // all-reduce over peer memory + update: reads both loss slots and waits for the peers, so never beside the forward
+        if (with_update == 2 && dp_update(group, lr, mu, st)) return -1;
     } else if (mode == 2) {
         { Range r("madstereo/backward_full"); if (backward(2, 0, st)) return -1; }
         Range r("madstereo/update");

@@ -85,7 +85,14 @@ struct Engine {
     int n_disp;
     TView g_disp;
     float* wT; size_t wT_floats;     // transposed-weight scratch
-    float* gemm_part;                            // split-K partial sums of the CUDA-core conv (conv_gemm) on small maps
+    // split-K scratch: partial sums of conv_bf (with its self-resetting tickets) and of the CUDA-core conv (conv_gemm) on
+    // small maps.  Set 0 serves the forward and every serial pass; set 1 the MAD train op that runs beside the rest of the
+    // forward (mad_branch) -- it aliases set 0 where no such branch can run, and set 0's conv_gemm partials where no MAD
+    // module's dgrad runs on conv_gemm.  Both sets have the same sizes, so the kernels split K the same way on either.
+    struct SplitK { float* bf_part; unsigned int* bf_tickets; float* gemm_part; };
+    SplitK splitk[2];
+    int on_branch;                   // which set the launches being enqueued use
+    const SplitK& sk() const { return splitk[on_branch]; }
     bool weights_dirty;
     // refreshes the tensor-core weight tiles of a module's layers right after its momentum update (-1 = all, after load/restore)
     int prep_layers(int group, cudaStream_t st);
@@ -102,6 +109,11 @@ struct Engine {
     cudaStream_t wstream; cudaEvent_t ev_fork, ev_join; bool wstream_dirty;
     int fork_wgrad(cudaStream_t st, cudaStream_t* ws);
     int join_wgrad(cudaStream_t st);
+    // MAD train op on a branch of the captured step: module g's loss, backward and update read only forward tensors that
+    // exist once its disparity head has run (level 6-g's disp6, or context7 for the last module) and that nothing later in
+    // the forward writes, so they run on `bstream` beside the rest of the forward.  MADNet only, and off while profiling
+    bool mad_branch(int mode, int group) const;
+    cudaStream_t bstream; cudaEvent_t ev_bfork, ev_bjoin;
     int backward_impl(int mode, int group, cudaStream_t st);
     int run(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st);
     int run_eager(int mode, int group, int disp_mask, int with_update, float lr, float mu, float gscale, cudaStream_t st);
@@ -113,7 +125,6 @@ struct Engine {
     std::set<const float*> fresh;                  // planes already written by a conv epilogue in the current pass
     std::vector<BfPrepJob> bf_jobs; std::vector<int> bf_job_begin, bf_job_end;
     BfPrepJob* bf_jobs_dev; size_t bf_max_total;
-    float* bf_part; unsigned int* bf_tickets;
     ActPlanes wg_xp; size_t wg_xp_halfs;              // bf16 scratch planes: forward activations re-split for the weight gradient
     float act_scale;                                  // power-of-two scale of the fp16 forward planes (per network)
     int ensure_planes(const TView& v, const ActPlanes* pl, cudaStream_t st);
@@ -133,6 +144,7 @@ struct Engine {
     float* wg_ws; size_t wg_ws_floats;
     float* rs_tmp; size_t rs_tmp_floats;
     float* loss_ws; size_t loss_ws_floats;
+    float* loss_full_ws;             // full-resolution loss without gradient, apart from loss_ws (nullptr: shares loss_ws)
     unsigned char* u8_stage;         // 2 x B*H*W*3 bytes: uint8 input staging (set_input_u8)
     // optimizer of update(): 0 = momentum SGD (Mo = accumulator), 1 = Adam (Mo = first moment, adam_v = second moment,
     // adam_powers = device [beta1_power, beta2_power] shared by every train op); caller-owned storage (ms_engine_set_optimizer)
@@ -181,7 +193,9 @@ struct Engine {
     int set_input_u8_resized(const unsigned char* left, const unsigned char* right, int h, int w, int rh, int rw, cudaStream_t st);
     int set_optimizer(int kind, float beta1, float beta2, float eps, float* v, float* powers);
     void drop_graphs();
-    int forward(int disp_mask, cudaStream_t st);
+    // branch != nullptr: right after module fork_group's disparity head, `branch` waits for `st`, and that module's
+    // full-resolution disparity is resized on `branch`
+    int forward(int disp_mask, cudaStream_t st, int fork_group = -1, cudaStream_t branch = nullptr);
     int loss(int which, int with_grad, int slot, float grad_scale, cudaStream_t st);
     int backward(int mode, int group, cudaStream_t st);     // mode 1 = MAD(group), 2 = FULL
     int update(int group, float lr, float mu, float gscale, cudaStream_t st);

@@ -169,7 +169,7 @@ int Engine::deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, co
         p.accumulate = dx_acc;
         prof_begin(CAT_CONV_DGRAD, st, li);
         // (an accumulating launch would leave dx's own planes stale: it writes none)
-        const int rc = P.dgrad == ConvPlan::DGRAD_BF ? conv_bf(p, *P.dp, P.tiles[1], nullptr, bf_part, bf_tickets, st) : conv_gemm(p, st);
+        const int rc = P.dgrad == ConvPlan::DGRAD_BF ? conv_bf(p, *P.dp, P.tiles[1], nullptr, sk().bf_part, sk().bf_tickets, st) : conv_gemm(p, st);
         planes_written(*dx, P.dxp, false);
         prof_end(st);
         prof_note((double)x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);

@@ -164,10 +164,13 @@ __global__ void loss_final_kernel(const float* __restrict__ l1_partial, int n1, 
     if (threadIdx.x == 0) *loss = (float)(0.85 * sm2[0] * inv_nw + 0.15 * sm1[0] * inv_np);
 }
 
-size_t loss_workspace_floats(int B, int H, int W) {
+// workspace layout: [xw 3n | dxw 3n | L1 partials | SSIM partials | coef 9n]; the gradient coefficients come last so that
+// a pass without gradient needs only loss_value_workspace_floats
+size_t loss_value_workspace_floats(int B, int H, int W) {
     size_t n = (size_t)B * H * W;
-    return n * 3 * 2 + n * 9 + 2 * (n / LB + 2) + 64;
+    return n * 3 * 2 + 2 * (n / LB + 2) + 64;
 }
+size_t loss_workspace_floats(int B, int H, int W) { return loss_value_workspace_floats(B, H, W) + (size_t)B * H * W * 9; }
 
 int reproj_loss(const ReprojLoss& p, cudaStream_t st) {
     MS_REQUIRE(p.H >= 3 && p.W >= 3, "reproj_loss: image too small for 3x3 SSIM windows");
@@ -175,10 +178,10 @@ int reproj_loss(const ReprojLoss& p, cudaStream_t st) {
     const size_t nwin = (size_t)p.B * (p.H - 2) * (p.W - 2);
     float* xw = p.workspace;
     float* dxw = xw + n * 3;
-    float* coef = dxw + n * 3;
-    float* l1p = coef + n * 9;
+    float* l1p = dxw + n * 3;
     const int nb1 = (int)cdivz(n, LB), nb2 = (int)cdivz(nwin, LB);
     float* ssp = l1p + nb1 + 1;
+    float* coef = ssp + nb2 + 1;
     const double inv_np = 1.0 / ((double)n * 3.0), inv_nw = 1.0 / ((double)nwin * 3.0);
     launch_k(loss_warp_kernel, dim3(nb1), dim3(LB), 0, st, p, xw, dxw, l1p);
     launch_k(loss_ssim_kernel, dim3(nb2), dim3(LB), 0, st, p, xw, p.ddisp ? coef : nullptr, ssp, (float)(0.85 * inv_nw));
