@@ -180,6 +180,14 @@ int ms_momentum_update(float* w, const float* g, float* m, size_t n, float lr, f
 int ms_adam_update(float* w, const float* g, float* m, float* v, float* powers, size_t n, float lr, float beta1, float beta2,
                    float eps, float grad_scale, void* stream);
 
+/* Stereo rectification of raw camera frames (no reference counterpart: the reference's grabbers deliver rectified
+ * frames): uint8 DEVICE frames src [B,h,w,3] -> dst [B,h,w,3] through the remap table map [h,w,2] float32, map[y,x] =
+ * (src_x, src_y), shared by the B frames (cv2.initUndistortRectifyMap(..., CV_32FC1) stacked; 8-byte aligned).  Per output
+ * pixel: the four taps at floor(src) are blended bilinearly in fp32, a tap outside the frame reads 0 (cv2.BORDER_CONSTANT),
+ * the result is rounded to nearest with ties to even and clamped to [0, 255]; a NaN entry or one outside
+ * [-1, w] x [-1, h] gives 0. */
+int ms_rectify_u8(const unsigned char* src, const float* map, int B, int h, int w, unsigned char* dst, void* stream);
+
 /* Replaces preprocessing.pad_image REFLECT padding (Data_utils/preprocessing.py:7-29). */
 int ms_pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int Hp, int Wp, int dst_cs,
                    float scale, float bias, void* stream);
@@ -214,6 +222,12 @@ int ms_engine_set_input_u8(void* e, const unsigned char* left, const unsigned ch
  * ms_engine_set_input_u8 bit for bit. */
 int ms_engine_set_input_u8_resized(void* e, const unsigned char* left, const unsigned char* right, int src_h, int src_w,
                                    int resize_h, int resize_w, void* stream);
+/* Rectification of ms_engine_set_input_u8_resized: from now on its frames, which must then be [B,src_h,src_w,3], are first
+ * rectified as ms_rectify_u8 describes (map_left for the left camera, map_right for the right, both [src_h,src_w,2]) into
+ * scratch, and the rescale + crop reads them from there.  Tables and scratch (>= 2*B*src_h*src_w*3 bytes) are caller-owned
+ * device memory that must outlive their use.  map_left == map_right == NULL turns rectification off. */
+int ms_engine_set_rectification(void* e, const float* map_left, const float* map_right, int src_h, int src_w,
+                                unsigned char* scratch, size_t scratch_bytes);
 /* Optimizer of ms_engine_update / ms_engine_run (with_update=1).  kind 0 = tf.train.MomentumOptimizer (default,
  * Stereo_Online_Adaptation.py:85), 1 = tf.train.AdamOptimizer (Demo/demo_model.py:163) as ms_adam_update describes:
  * m lives in the momentum arena, v_arena holds n_param_floats floats (16-byte aligned), powers is a device float[2]

@@ -4,12 +4,15 @@ The reference's flags are kept flag for flag; `-1` disables --imageShape or --cr
 disabled the network runs at the camera size).  Additions for headless machines: --output DIR writes the displayed
 disparity image of every frame and a log.csv (step, loss, module, reset, step ms) instead of opening windows, and
 --maxFrames N stops after N frames.  The `ImageList` grabber replays a list file; --cameraConfig then names a JSON file
-{"list": "<left;right list>", "fps": <frames per second, 0 = no pacing>}.
+{"list": "<left;right list>", "fps": <frames per second, 0 = no pacing>}.  Any camera's configuration may also name
+"calibration": "<stereo calibration file>" (madstereo.rectify) when its frames are raw: they are then rectified on the
+device before the rescale.
 
     python Demo/Live_Adaptation_Demo.py --cameraName ImageList --cameraConfig cfg.json --weights ckpt/MADNet/kitti \\
         --mode MAD --blockConfig block_config/MadNet_full.json --output out --maxFrames 300
 """
 import argparse
+import json
 import os
 import queue
 import sys
@@ -70,8 +73,11 @@ def main(args):
         raise SystemExit('camera grabber {} is not available here (available: {})'.format(
             args.cameraName, ', '.join(grabber.get_available_camera())))
     camera_cls = grabber._GRABBER_FACTORY[args.cameraName]
+    calibration = None
     if getattr(camera_cls, 'needs_config', True):
         assert os.path.exists(args.cameraConfig), 'camera configuration {} not found'.format(args.cameraConfig)
+        with open(args.cameraConfig) as f_in:
+            calibration = json.load(f_in).get('calibration')
 
     # setup shared queue for the grabbed frames
     camera_frames = queue.Queue(1)
@@ -88,7 +94,8 @@ def main(args):
         SSIMTh=args.SSIMTh,
         mode=args.mode,
         output=args.output,
-        max_frames=args.maxFrames)
+        max_frames=args.maxFrames,
+        calibration=calibration)
     gg = grabber.get_camera(args.cameraName, camera_frames, config=args.cameraConfig, framerate=30)
 
     print('Threads ready to start')

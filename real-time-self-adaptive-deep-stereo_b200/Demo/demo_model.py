@@ -2,7 +2,8 @@
 
 The TF graph of the reference (input rescale + crop :72-86, network :88-109, Adam train ops :111-170, restore :184-217)
 becomes `Nets.get_stereo_net` + `OnlineAdaptation(optimizer='adam')`; the camera frames go to the device as uint8 and are
-rescaled / cropped there (`StereoEngine.set_resize`).  The loop (:233-284) is kept as the reference runs it, quirks
+rescaled / cropped there (`StereoEngine.set_resize`), after an on-device rectification when the camera is calibrated
+(`StereoEngine.set_rectification`).  The loop (:233-284) is kept as the reference runs it, quirks
 included (see `run`).
 """
 import json
@@ -85,12 +86,13 @@ class RealTimeStereo(threading.Thread):
 
     def __init__(self, camera_buffer, model_name='MADNet', weight_path=None, learning_rate=0.0001,
                  block_config_path='../block_config/MadNet_full.json', image_shape=[480, 640], crop_shape=[None, None],
-                 SSIMTh=0.5, mode='MAD', output=None, max_frames=None, build=None, log=print):
+                 SSIMTh=0.5, mode='MAD', output=None, max_frames=None, calibration=None, build=None, log=print):
         """camera_buffer: queue of [2,h,w,3] uint8 frames (grabber.END_OF_STREAM ends the run); weight_path: initial
         weights (required: the TF random initialisers are not reproduced); image_shape / crop_shape: [None, None]
         disables the rescale / the crop; output: directory for the displayed disparity of every frame and log.csv (no
-        windows are opened); max_frames: stop after this many frames; build(height, width) -> (adapt, fetch) replaces
-        build_engine (tests)."""
+        windows are opened); max_frames: stop after this many frames; calibration: stereo calibration file
+        (madstereo.rectify) of a camera that delivers raw frames, which are then rectified on the device;
+        build(height, width) -> (adapt, fetch) replaces build_engine (tests)."""
         threading.Thread.__init__(self)
         assert mode in MODES
         if weight_path is None:
@@ -108,6 +110,11 @@ class RealTimeStereo(threading.Thread):
         self._max_frames = max_frames
         self._build = build
         self._log = log
+        self._calibration = None
+        if calibration is not None:
+            from madstereo.rectify import load_calibration
+            self._calibration = load_calibration(calibration)
+        self._rectifying = False
         self._stop_flag = False
         self._adapt = None
         self.error = None
@@ -136,6 +143,13 @@ class RealTimeStereo(threading.Thread):
         self._expected_loss = 0
         self._last_trained_blocks = 0
         print('Network Ready')
+
+    def _setup_rectification(self, frame_size):
+        """Rectification tables for the camera's frame size (refused when it is not the calibrated size), on the engine."""
+        from madstereo.rectify import rectification_maps
+        map_left, map_right = rectification_maps(self._calibration, frame_size)
+        self._adapt.engine.set_rectification(map_left, map_right)
+        self._rectifying = True
 
     def _setup_gui(self):
         import cv2
@@ -175,6 +189,8 @@ class RealTimeStereo(threading.Thread):
             right_frame = frames[1:]
             if self._adapt is None:
                 self._setup(network_shape(self._image_shape, self._crop_shape, left_frame.shape[1:3]))
+            if self._calibration is not None and not self._rectifying:
+                self._setup_rectification(left_frame.shape[1:3])
 
             # the module is drawn from softmax(sample_distribution) inside OnlineAdaptation.step (:243-247)
             self._adapt.sample_distribution = self._sample_distribution.copy()

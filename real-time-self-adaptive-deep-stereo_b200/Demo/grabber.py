@@ -96,7 +96,8 @@ class ImageGrabber(threading.Thread, metaclass=abc.ABCMeta):
 class ImageList(ImageGrabber):
     """Replays a `left;right[;...]` list file (the format of Data_utils.data_reader) as uint8 RGB frames.
 
-    config: JSON file {"list": path, "fps": frames per second}; fps 0 (or absent) means no pacing."""
+    config: JSON file {"list": path, "fps": frames per second}; fps 0 (or absent) means no pacing.  A "calibration" key
+    is read by the demo, not here: the listed frames are then raw and are rectified on the device."""
     _name = 'ImageList'
 
     def _connect_to_camera(self):

@@ -378,6 +378,10 @@ int ms_adam_update(float* w, const float* g, float* m, float* v, float* powers, 
     return adam_update(w, g, m, v, powers, n, lr, beta1, beta2, eps, grad_scale, S(stream));
 }
 
+int ms_rectify_u8(const unsigned char* src, const float* map, int B, int h, int w, unsigned char* dst, void* stream) {
+    return rectify_u8(src, nullptr, map, nullptr, B, h, w, dst, nullptr, S(stream));
+}
+
 int ms_pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int Hp, int Wp, int dst_cs, float scale,
                    float bias, void* stream) {
     return pad_reflect(src, B, H, W, C, dst, Hp, Wp, dst_cs, scale, bias, S(stream));
@@ -468,6 +472,10 @@ int ms_engine_set_input_u8(void* h, const unsigned char* left, const unsigned ch
 int ms_engine_set_input_u8_resized(void* h, const unsigned char* left, const unsigned char* right, int src_h, int src_w,
                                    int resize_h, int resize_w, void* stream) {
     return static_cast<Engine*>(h)->set_input_u8_resized(left, right, src_h, src_w, resize_h, resize_w, S(stream));
+}
+int ms_engine_set_rectification(void* h, const float* map_left, const float* map_right, int src_h, int src_w,
+                                unsigned char* scratch, size_t scratch_bytes) {
+    return static_cast<Engine*>(h)->set_rectification(map_left, map_right, src_h, src_w, scratch, scratch_bytes);
 }
 int ms_engine_set_optimizer(void* h, int kind, float beta1, float beta2, float eps, float* v_arena, float* powers) {
     return static_cast<Engine*>(h)->set_optimizer(kind, beta1, beta2, eps, v_arena, powers);

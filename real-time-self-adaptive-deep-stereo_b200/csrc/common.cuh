@@ -185,6 +185,10 @@ int u8_to_f32(const unsigned char* src, float* dst, size_t n, cudaStream_t st);
 // uint8 [B,h,w,3] left + right frames -> fp32 [B,H,W,3]: legacy bilinear rescale to (rh, rw), then centre crop / zero pad
 int u8_resize_crop(const unsigned char* left, const unsigned char* right, int B, int h, int w, int rh, int rw, float* dst_left,
                    float* dst_right, int H, int W, cudaStream_t st);
+// uint8 [B,h,w,3] frames -> rectified uint8 [B,h,w,3] through per-camera [h,w,2] float32 remap tables (bilinear, constant 0
+// border); right, map_right, dst_right all null = the left camera only
+int rectify_u8(const unsigned char* left, const unsigned char* right, const float* map_left, const float* map_right, int B,
+               int h, int w, unsigned char* dst_left, unsigned char* dst_right, cudaStream_t st);
 
 // loss (loss.cu)
 struct ReprojLoss {

@@ -301,4 +301,55 @@ int u8_resize_crop(const unsigned char* left, const unsigned char* right, int B,
     return check_launch("u8_resize_crop");
 }
 
+// Stereo rectification of raw camera frames, what cv2.remap(frame, map, INTER_LINEAR, BORDER_CONSTANT 0) does, with the
+// taps blended in fp32 instead of OpenCV's 1/32-pixel fixed point.  map[y, x] = (src_x, src_y), [h,w,2] float32 (the
+// tables of cv2.initUndistortRectifyMap(..., CV_32FC1) stacked), one per camera and shared by the frames of a batch.
+// A tap outside the frame reads 0; the blend is rounded to nearest, ties to even, as saturate_cast<uchar> does.  A map
+// entry that is NaN or outside [-1, w] x [-1, h] gives 0 without forming an index (every tap of such an entry would be
+// outside anyway).  One thread per output pixel of either frame (left: first B*h*w threads; ncam 1 = left only).
+__global__ void rectify_u8_kernel(const unsigned char* __restrict__ left, const unsigned char* __restrict__ right,
+                                  const float2* __restrict__ map_l, const float2* __restrict__ map_r, int ncam, int B,
+                                  int h, int w, unsigned char* __restrict__ dl, unsigned char* __restrict__ dr) {
+    pdl_prologue();
+    const size_t hw = (size_t)h * w, per = (size_t)B * hw;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)ncam * per) return;
+    const bool is_r = i >= per;
+    const size_t j = is_r ? i - per : i;
+    const float2 m = (is_r ? map_r : map_l)[j % hw];
+    unsigned char* d = (is_r ? dr : dl) + j * 3;
+    if (!(m.x >= -1.f && m.x <= (float)w && m.y >= -1.f && m.y <= (float)h)) { d[0] = 0; d[1] = 0; d[2] = 0; return; }
+    const float fx0 = floorf(m.x), fy0 = floorf(m.y);
+    const int x0 = (int)fx0, y0 = (int)fy0;
+    const float fx = m.x - fx0, fy = m.y - fy0;
+    const unsigned char* s = (is_r ? right : left) + (j / hw) * hw * 3;
+    const bool in_x0 = x0 >= 0 && x0 < w, in_x1 = x0 + 1 < w, in_y0 = y0 >= 0 && y0 < h, in_y1 = y0 + 1 < h;
+    const unsigned char* r0 = s + (size_t)(in_y0 ? y0 : 0) * w * 3;
+    const unsigned char* r1 = s + (size_t)(in_y1 ? y0 + 1 : 0) * w * 3;
+    const int c0 = (in_x0 ? x0 : 0) * 3, c1 = (in_x1 ? x0 + 1 : 0) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float tl = in_y0 && in_x0 ? (float)r0[c0 + c] : 0.f, tr = in_y0 && in_x1 ? (float)r0[c1 + c] : 0.f;
+        const float bl = in_y1 && in_x0 ? (float)r1[c0 + c] : 0.f, br = in_y1 && in_x1 ? (float)r1[c1 + c] : 0.f;
+        const float top = tl + (tr - tl) * fx;
+        const float bot = bl + (br - bl) * fx;
+        d[c] = (unsigned char)min(max(__float2int_rn(top + (bot - top) * fy), 0), 255);
+    }
+}
+
+int rectify_u8(const unsigned char* left, const unsigned char* right, const float* map_left, const float* map_right, int B,
+               int h, int w, unsigned char* dst_left, unsigned char* dst_right, cudaStream_t st) {
+    MS_REQUIRE(B >= 1 && h >= 1 && w >= 1, "rectify_u8: bad geometry");
+    MS_REQUIRE(left && map_left && dst_left, "rectify_u8: null pointer");
+    MS_REQUIRE(!right == !map_right && !right == !dst_right, "rectify_u8: the right frame needs its own map and output");
+    MS_REQUIRE(((reinterpret_cast<uintptr_t>(map_left) | reinterpret_cast<uintptr_t>(map_right)) & 7) == 0,
+               "rectify_u8: maps must be 8-byte aligned");
+    const int ncam = right ? 2 : 1;
+    const size_t total = (size_t)ncam * B * h * w;
+    launch_k(rectify_u8_kernel, dim3((unsigned)cdivz(total, 256)), dim3(256), 0, st, left, right,
+             reinterpret_cast<const float2*>(map_left), reinterpret_cast<const float2*>(map_right), ncam, B, h, w, dst_left,
+             dst_right);
+    return check_launch("rectify_u8");
+}
+
 }  // namespace ms

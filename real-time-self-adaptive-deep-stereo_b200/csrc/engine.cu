@@ -47,6 +47,7 @@ Engine::Engine()
     bf_jobs_dev = nullptr; bf_max_total = 0;
     dp_rank = 0; dp_world = 1; dp_connected = false; dp_xbuf = nullptr; dp_state = nullptr; dp_cap_floats = 0;
     opt_kind = 0; adam_b1 = adam_b2 = adam_eps = 0.f; adam_v = nullptr; adam_powers = nullptr;
+    rect_map_l = rect_map_r = nullptr; rect_h = rect_w = 0; rect_scratch = nullptr;
 }
 
 void Engine::drop_graphs() {
@@ -582,11 +583,37 @@ int Engine::set_input_u8(const unsigned char* left, const unsigned char* right, 
     return u8_to_f32(right_stage, rr.p, n, st);
 }
 
-// uint8 device frames [B,h,w,3] at camera size: rescale to (rh, rw) and centre crop / zero pad to (H, W) in one pass
+// uint8 device frames [B,h,w,3] at camera size: rescale to (rh, rw) and centre crop / zero pad to (H, W) in one pass;
+// with rectification set, the frames are first rectified into the scratch and the rescale reads them from there
 int Engine::set_input_u8_resized(const unsigned char* left, const unsigned char* right, int h, int w, int rh, int rw,
                                  cudaStream_t st) {
     MS_REQUIRE(bound, "engine not bound");
+    if (rect_map_l) {
+        MS_REQUIRE(h == rect_h && w == rect_w, "set_input_u8_resized: frames are " + std::to_string(h) + "x" + std::to_string(w) +
+                                               ", the rectification tables " + std::to_string(rect_h) + "x" + std::to_string(rect_w));
+        unsigned char* rl = rect_scratch;
+        unsigned char* rr = rect_scratch + (size_t)B * h * w * 3;
+        if (rectify_u8(left, right, rect_map_l, rect_map_r, B, h, w, rl, rr, st)) return -1;
+        left = rl; right = rr;
+    }
     return u8_resize_crop(left, right, B, h, w, rh, rw, tensors["raw_left"].p, tensors["raw_right"].p, H, W, st);
+}
+
+int Engine::set_rectification(const float* map_left, const float* map_right, int h, int w, unsigned char* scratch,
+                              size_t scratch_bytes) {
+    if (!map_left && !map_right) {
+        rect_map_l = rect_map_r = nullptr; rect_h = rect_w = 0; rect_scratch = nullptr;
+        return 0;
+    }
+    MS_REQUIRE(map_left && map_right, "set_rectification: both cameras need a table (two NULL tables turn it off)");
+    MS_REQUIRE(h >= 1 && w >= 1, "set_rectification: bad table size");
+    MS_REQUIRE(((reinterpret_cast<uintptr_t>(map_left) | reinterpret_cast<uintptr_t>(map_right)) & 7) == 0,
+               "set_rectification: tables must be 8-byte aligned");
+    const size_t need = 2 * (size_t)B * h * w * 3;
+    MS_REQUIRE(scratch && scratch_bytes >= need,
+               "set_rectification: the scratch must hold both rectified frames (" + std::to_string(need) + " bytes)");
+    rect_map_l = map_left; rect_map_r = map_right; rect_h = h; rect_w = w; rect_scratch = scratch;
+    return 0;
 }
 
 int Engine::prep_layers(int group, cudaStream_t st) {

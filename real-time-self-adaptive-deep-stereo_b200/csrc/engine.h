@@ -146,6 +146,11 @@ struct Engine {
     float* loss_ws; size_t loss_ws_floats;
     float* loss_full_ws;             // full-resolution loss without gradient, apart from loss_ws (nullptr: shares loss_ws)
     unsigned char* u8_stage;         // 2 x B*H*W*3 bytes: uint8 input staging (set_input_u8)
+    // rectification of set_input_u8_resized (ms_engine_set_rectification): [rect_h,rect_w,2] remap table per camera and a
+    // 2 x B*rect_h*rect_w*3 byte scratch for the rectified frames, caller-owned; rect_map_l == nullptr: off
+    const float* rect_map_l; const float* rect_map_r;
+    int rect_h, rect_w;
+    unsigned char* rect_scratch;
     // optimizer of update(): 0 = momentum SGD (Mo = accumulator), 1 = Adam (Mo = first moment, adam_v = second moment,
     // adam_powers = device [beta1_power, beta2_power] shared by every train op); caller-owned storage (ms_engine_set_optimizer)
     int opt_kind;
@@ -191,6 +196,7 @@ struct Engine {
     int set_input(const float* left, const float* right, cudaStream_t st);
     int set_input_u8(const unsigned char* left, const unsigned char* right, cudaStream_t st);
     int set_input_u8_resized(const unsigned char* left, const unsigned char* right, int h, int w, int rh, int rw, cudaStream_t st);
+    int set_rectification(const float* map_left, const float* map_right, int h, int w, unsigned char* scratch, size_t scratch_bytes);
     int set_optimizer(int kind, float beta1, float beta2, float eps, float* v, float* powers);
     void drop_graphs();
     // branch != nullptr: right after module fork_group's disparity head, `branch` waits for `st`, and that module's

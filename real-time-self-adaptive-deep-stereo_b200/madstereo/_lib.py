@@ -58,6 +58,7 @@ _SIGS = {
     'ms_reproj_loss': (I, [P, P, P, I, I, I, P, P, P, F, P]),
     'ms_momentum_update': (I, [P, P, P, Z, F, F, F, P]),
     'ms_adam_update': (I, [P, P, P, P, P, Z, F, F, F, F, F, P]),
+    'ms_rectify_u8': (I, [P, P, I, I, I, P, P]),
     'ms_pad_reflect': (I, [P, I, I, I, I, P, I, I, I, F, F, P]),
     'ms_engine_create': (P, [c_char_p, I, I, I, I, I, I]),
     'ms_engine_destroy': (I, [P]),
@@ -71,6 +72,7 @@ _SIGS = {
     'ms_engine_set_input': (I, [P, P, P, P]),
     'ms_engine_set_input_u8': (I, [P, P, P, P]),
     'ms_engine_set_input_u8_resized': (I, [P, P, P, I, I, I, I, P]),
+    'ms_engine_set_rectification': (I, [P, P, P, I, I, P, Z]),
     'ms_engine_set_optimizer': (I, [P, I, F, F, F, P, P]),
     'ms_engine_set_gt': (I, [P, P, P]),
     'ms_engine_set_proxy': (I, [P, P, P]),

@@ -66,6 +66,7 @@ class StereoEngine:
         self.optimizer = 'momentum'
         self.resize_shape = None      # set_resize(): None = uint8 frames must be [B,H,W,3]; else (rh, rw), -1 = no rescale
         self._rs_stage = None
+        self._rect = None             # set_rectification(): (left table, right table, scratch) the engine reads per frame
 
     def _on_device(self):
         """Context that makes this engine's GPU current -- a no-op object when it already is (the per-frame calls of a
@@ -174,7 +175,41 @@ class StereoEngine:
             image_shape = tuple(int(v) for v in image_shape)
             if len(image_shape) != 2 or (min(image_shape) < 1 and image_shape != (-1, -1)):
                 raise MadStereoError('set_resize: image_shape must be (height, width) or (-1, -1), got %r' % (image_shape,))
+        elif self._rect is not None:
+            raise MadStereoError('set_resize(None): turn rectification off first (set_rectification(None))')
         self.resize_shape = image_shape
+
+    def set_rectification(self, map_left, map_right=None):
+        """Rectify the uint8 camera frames of the set_resize() path on the device before they are rescaled: map_left /
+        map_right are float32 [h,w,2] remap tables, map[y, x] = (src_x, src_y), as cv2.initUndistortRectifyMap(...,
+        cv2.CV_32FC1) returns them stacked (madstereo.rectify builds them from a stereo calibration); frames must then be
+        [B,h,w,3].  Bilinear, 0 outside the frame, rounded back to uint8 (what cv2.remap gives, up to OpenCV's 1/32-pixel
+        fixed point).  None turns rectification off."""
+        if map_left is None:
+            with self._on_device():
+                check(self._lib.ms_engine_set_rectification(self._h, c_void_p(0), c_void_p(0), 0, 0, c_void_p(0), 0),
+                      'set_rectification')
+            self._rect = None
+            return
+        if self.resize_shape is None:
+            raise MadStereoError('set_rectification: rectification applies to the set_resize() input path; call set_resize first')
+        maps = []
+        for m in (map_left, map_right):
+            if m is None:
+                raise MadStereoError('set_rectification: each camera needs a table')
+            m = torch.as_tensor(m)
+            if m.dtype != torch.float32 or m.dim() != 3 or m.shape[2] != 2:
+                raise MadStereoError('set_rectification: tables must be float32 [h,w,2], got %s %s' % (m.dtype, tuple(m.shape)))
+            maps.append(m.to(self.device).contiguous())
+        if maps[0].shape != maps[1].shape:
+            raise MadStereoError('set_rectification: left %s and right %s tables differ in size'
+                                 % (tuple(maps[0].shape), tuple(maps[1].shape)))
+        h, w = int(maps[0].shape[0]), int(maps[0].shape[1])
+        scratch = torch.empty(2 * self.B * h * w * 3, dtype=torch.uint8, device=self.device)
+        with self._on_device():
+            check(self._lib.ms_engine_set_rectification(self._h, _ptr(maps[0]), _ptr(maps[1]), h, w, _ptr(scratch),
+                                                        scratch.numel()), 'set_rectification')
+        self._rect = (maps[0], maps[1], scratch)      # the engine reads them on every frame
 
     def _u8_source(self, x):
         """uint8 [B,h,w,3] frame -> contiguous CUDA tensor on this engine's device (host frames are copied on the current

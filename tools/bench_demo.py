@@ -2,7 +2,8 @@
 
   * steady-state adaptation steps per second at 320x512 (the demo's crop) for MADNet MAD and FULL, with Adam and with
     momentum, the four configurations alternated within one call;
-  * the uint8 rescale + crop kernel for a 720p frame pair -> 480x640 -> 320x512, device-resident frames;
+  * the uint8 rescale + crop kernel for a 720p and a 1080p frame pair -> 480x640 -> 320x512, device-resident frames,
+    alone and after on-device rectification, next to host cv2.remap of the same pair (what a grabber would otherwise do);
   * the demo itself (Demo/Live_Adaptation_Demo.py, MAD, Adam) on an ImageList of synthetic 480x640 pairs at fps 0, with
     --output: frames per second including decode, host display copies, colormap and PNG writes.
 
@@ -67,13 +68,34 @@ def time_steps(ad, lt, rt, steps):
     return steps / (time.perf_counter() - t0)
 
 
-def time_resize(iters=500):
+def camera_pair(h, w, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    return [torch.randint(0, 256, (1, h, w, 3), dtype=torch.uint8, generator=g) for _ in range(2)]
+
+
+def rectification_tables(h, w):
+    """Tables of a plausible raw stereo rig (barrel distortion, a 2-degree rotation between the cameras)."""
+    import cv2
+    K = np.array([[0.7 * w, 0, w / 2], [0, 0.7 * w, h / 2], [0, 0, 1]])
+    D = np.array([-0.3, 0.1, 1e-3, -5e-4, -0.02])
+    R, _ = cv2.Rodrigues(np.radians([1.0, -2.0, 0.5]))
+    r1, r2, p1, p2 = cv2.stereoRectify(K, D, K, D, (w, h), R, np.array([-0.12, 0.002, 0.001]),
+                                       flags=cv2.CALIB_ZERO_DISPARITY, alpha=0)[:4]
+    return [np.stack(cv2.initUndistortRectifyMap(K, D, r, p, (w, h), cv2.CV_32FC1), -1) for r, p in ((r1, p1), (r2, p2))]
+
+
+def time_input(h, w, tables=None, iters=500):
+    """Time of the camera-frame input path (optional rectify, rescale to 480x640, crop to 320x512) for one pair, in us:
+    (back to back: events around `iters` calls, whatever bounds them, host or device, with frames and tables left in
+    L2 from the previous call; cold: device time between events around each call, after a write of 128 MB that evicts
+    L2 and keeps the device busy while the host enqueues the call, as a camera frame arriving after an adaptation
+    step finds it)."""
     from madstereo.engine import StereoEngine
     eng = StereoEngine('MADNet', 1, 320, 512)
     eng.set_groups([]); eng.bind(); eng.set_resize((480, 640))
-    g = torch.Generator().manual_seed(0)
-    l = torch.randint(0, 256, (1, 720, 1280, 3), dtype=torch.uint8, generator=g).cuda()
-    r = torch.randint(0, 256, (1, 720, 1280, 3), dtype=torch.uint8, generator=g).cuda()
+    if tables is not None:
+        eng.set_rectification(*tables)
+    l, r = (x.cuda() for x in camera_pair(h, w))
     for _ in range(20):
         eng.set_input(l, r)
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -82,7 +104,50 @@ def time_resize(iters=500):
         eng.set_input(l, r)
     b.record()
     b.synchronize()
-    return 1e3 * a.elapsed_time(b) / iters
+    warm = 1e3 * a.elapsed_time(b) / iters
+    flush = torch.empty(32 << 20, dtype=torch.float32, device='cuda')
+    cold = []
+    for _ in range(iters // 5):
+        flush.fill_(1.0)
+        a.record()
+        eng.set_input(l, r)
+        b.record()
+        b.synchronize()
+        cold.append(1e3 * a.elapsed_time(b))
+    return warm, float(np.median(cold))
+
+
+def time_host_remap(h, w, tables, iters=20):
+    """What a grabber that rectifies on the host spends per pair: two cv2.remap calls (OpenCV's own threads)."""
+    import cv2
+    l, r = (x[0].numpy() for x in camera_pair(h, w))
+    maps = [(t[..., 0].copy(), t[..., 1].copy()) for t in tables]
+    def pair():
+        return [cv2.remap(img, mx, my, cv2.INTER_LINEAR, borderMode=cv2.BORDER_CONSTANT) for img, (mx, my) in zip((l, r), maps)]
+    pair()
+    t0 = time.perf_counter()
+    for _ in range(iters):
+        pair()
+    return 1e6 * (time.perf_counter() - t0) / iters
+
+
+def input_paths():
+    """Rescale + crop alone and with rectification for a 720p and a 1080p pair, plus host cv2.remap of the same pair.
+    Traffic of the rectify pass: raw frames read, tables read, rectified frames written (then re-read by the rescale,
+    counted once more), in MB."""
+    import cv2
+    out = {'host_cv2_threads': cv2.getNumThreads()}
+    for name, (h, w) in (('720p', (720, 1280)), ('1080p', (1080, 1920))):
+        tables = rectification_tables(h, w)
+        warm, cold = time_input(h, w)
+        out['resize_%s_to_320x512_us' % name] = round(warm, 2)
+        out['resize_%s_to_320x512_cold_l2_us' % name] = round(cold, 2)
+        warm, cold = time_input(h, w, tables)
+        out['rectify_resize_%s_to_320x512_us' % name] = round(warm, 2)
+        out['rectify_resize_%s_to_320x512_cold_l2_us' % name] = round(cold, 2)
+        out['rectify_traffic_%s_mb' % name] = round(2 * h * w * (3 + 8 + 3 + 3) / 1e6, 1)
+        out['host_cv2_remap_%s_pair_us' % name] = round(time_host_remap(h, w, tables), 1)
+    return out
 
 
 def time_demo(frames):
@@ -136,7 +201,7 @@ def main():
     res['steps_per_s_320x512'] = {'%s_%s' % c: [round(v, 1) for v in rates[c]] for c in configs}
     del built
     torch.cuda.empty_cache()
-    res['resize_720p_to_320x512_us'] = round(time_resize(), 2)
+    res.update(input_paths())
     res.update(time_demo(a.demo_frames))
     print(json.dumps(res))
 
