@@ -243,6 +243,21 @@ int ms_engine_set_gt(void* e, const float* gt, void* stream);
  * Changing the loss drops the captured step graphs. */
 int ms_engine_set_proxy(void* e, const float* proxy, void* stream);
 int ms_engine_set_loss(void* e, int kind, float weight_full, float weight_module);
+/* MAD module losses at 1/scale resolution (the reference's --reprojectionScale, Stereo_Online_Adaptation.py:22-23,91-107
+ * and Stereo_Continual_Adaptation.py:95-112).  With h = H / scale, w = W / scale (integer division), the module loss of a
+ * MAD train op (ms_engine_loss slot 1, ms_engine_run mode 1) compares the module disparity resized to h x w (legacy
+ * bilinear, straight from its coarse head) with the frames resized to h x w, or with the proxy resized to h x w and
+ * divided by scale.  As in the reference, the disparity is NOT divided by scale: it stays in full-resolution pixels while
+ * it warps the 1/scale images (or meets the 1/scale proxy).  The full-resolution loss (slot 0), the FULL train op, the
+ * reward it feeds and EPE/bad3 do not change.
+ * Scratch: caller-owned device memory (16-byte aligned) of ms_engine_reprojection_scratch_floats(e, scale) floats, read
+ * and written by every MAD step until the scale changes; it holds the loss-resolution frames, proxy and disparity (engine
+ * tensors rs_left, rs_right, rs_proxy, rs_disp) and the resize tap tables.  scale 1 or a NULL scratch: full resolution,
+ * bit for bit as without the call.  Refused (negative code, ms_last_error) before bind, for scale < 1, for h or w < 3,
+ * for scale != 1 on DispNet (it has no MAD train ops) and for a scratch that is too small.  Changing the scale drops the
+ * captured step graphs.  ms_engine_reprojection_scratch_floats returns 0 for scale 1 and for a refused scale. */
+size_t ms_engine_reprojection_scratch_floats(void* e, int scale);
+int ms_engine_set_reprojection_scale(void* e, int scale, float* scratch, size_t scratch_floats);
 /* disp_mask bit i => materialise get_disparities()[i] (MADNet: D6,D5,D4,D3,D2ctx,full). */
 int ms_engine_forward(void* e, int disp_mask, void* stream);
 /* slot 0 = full-res loss fetched every frame (Stereo_Online_Adaptation.py:70,209), slot 1 = train loss */

@@ -6,7 +6,8 @@ disparities, weight 0.01 on the full-resolution loss / FULL train op :75,133 and
 op only every `--dilation` frames (:212), the reward recurrence with --decay / --uf (:232-234), the reset on --SSIMTh
 (:269-271) and the output files (`overall.csv`, `series.csv`, `histogram.csv`, `disparities/disparity_<step>.png`,
 `weights/`).  Underneath: Nets.get_stereo_net + madstereo.adaptation.OnlineAdaptation(loss='proxy', ...).step, the masked-L1
-loss is csrc/loss.cu:proxy_loss.  --reprojectionScale != 1 and --summary are not supported (as in the online driver).
+loss is csrc/loss.cu:proxy_loss.  --reprojectionScale s compares the MAD module disparities with the proxy resized to 1/s
+and divided by s (:95-112); --summary is accepted but not written (as in the online driver).
 
     python Stereo_Continual_Adaptation.py -l list.csv -o out --weights ckpt --modelName MADNet \
         --blockConfig block_config/MadNet_full.json --mode MAD --sampleMode PROBABILITY --dilation 1
@@ -69,7 +70,8 @@ def build_model(args, train_config):
         assert (len(stereo_net.get_disparities()[:-1]) == len(train_config))
     adapt = OnlineAdaptation(stereo_net, mode=args.mode, train_config=train_config, lr=args.lr, sample_mode=args.sampleMode,
                              num_blocks=args.numBlocks, fixed_id=args.fixedID, sample_frequency=args.sampleFrequency,
-                             ssim_th=args.SSIMTh, loss='proxy', decay=args.decay, uf=args.uf, dilation=args.dilation)
+                             ssim_th=args.SSIMTh, loss='proxy', decay=args.decay, uf=args.uf, dilation=args.dilation,
+                             reprojection_scale=args.reprojectionScale)
     return stereo_net, adapt
 
 
@@ -110,8 +112,7 @@ def write_outputs(args, avg_accumulator, d1_accumulator):
 def main(args, build=build_model):
     with open(args.blockConfig) as json_data:
         train_config = json.load(json_data)
-    if args.reprojectionScale != 1:
-        raise SystemExit('--reprojectionScale != 1 is not supported: the engine computes every loss at full resolution')
+    online.check_reprojection_scale(args)
     data_set = data_reader.dataset(args.list, batch_size=1, crop_shape=args.imageShape, num_epochs=1, augment=False,
                                    is_training=False, shuffle=False, proxies=True)
     stereo_net, adapt = build(args, train_config)

@@ -6,7 +6,8 @@ same loop (:176-253).  What changed underneath: the graph construction and `sess
 `madstereo.adaptation.OnlineAdaptation.step` (sampling, reward recurrence, reset and the CUDA step live there), the
 `tf.data` reader is Data_utils/data_reader.py (host thread + pinned buffers; the next frame's copy overlaps the current
 frame), `--weights` accepts a TensorFlow V2 checkpoint prefix or directory (read without TensorFlow) or an `.npz`, and
-TensorBoard summaries (`--summary`) are accepted but not written.
+TensorBoard summaries (`--summary`) are accepted but not written.  `--reprojectionScale s` computes the MAD module losses at
+1/s resolution as the reference does (:22-23, :91-107), disparity units included; it has no effect under FULL / NONE.
 
     python Stereo_Online_Adaptation.py -l list.csv -o out --weights ckpt/MADNet/kitti/weights.ckpt \\
         --modelName MADNet --blockConfig block_config/MadNet_full.json --mode MAD --sampleMode PROBABILITY
@@ -145,15 +146,24 @@ def build_model(args, train_config):
         assert (len(stereo_net.get_disparities()[:-1]) == len(train_config))
     adapt = OnlineAdaptation(stereo_net, mode=args.mode, train_config=train_config, lr=args.lr, sample_mode=args.sampleMode,
                              num_blocks=args.numBlocks, fixed_id=args.fixedID, sample_frequency=args.sampleFrequency,
-                             ssim_th=args.SSIMTh)
+                             ssim_th=args.SSIMTh, reprojection_scale=args.reprojectionScale)
     return stereo_net, adapt
+
+
+def check_reprojection_scale(args):
+    """--reprojectionScale must be >= 1, and MAD at s != 1 needs MADNet: DispNet has no MAD train ops on the engine (the
+    reference's own assert at :97 stops that combination too)."""
+    if args.reprojectionScale < 1:
+        raise SystemExit('--reprojectionScale must be >= 1, got %d' % args.reprojectionScale)
+    if args.reprojectionScale != 1 and args.mode == 'MAD' and args.modelName != 'MADNet':
+        raise SystemExit('--reprojectionScale %d with --mode MAD needs --modelName MADNet (%s has no MAD train ops)'
+                         % (args.reprojectionScale, args.modelName))
 
 
 def main(args, build=build_model):
     with open(args.blockConfig) as json_data:
         train_config = json.load(json_data)
-    if args.reprojectionScale != 1:
-        raise SystemExit('--reprojectionScale != 1 is not supported: the engine computes every loss at full resolution')
+    check_reprojection_scale(args)
     if len(args.imageShape) != 2:
         raise SystemExit('--imageShape takes two integers: height width')
 

@@ -490,6 +490,7 @@ int ms_engine_set_proxy(void* h, const float* proxy, void* stream) {
     Engine* e = static_cast<Engine*>(h);
     if (!e->bound) { set_error("engine not bound"); return -2; }
     MS_CHECK_CUDA(cudaMemcpyAsync(e->proxy, proxy, (size_t)e->B * e->H * e->W * sizeof(float), cudaMemcpyDefault, S(stream)));
+    e->rs_fresh = false;
     return 0;
 }
 int ms_engine_set_loss(void* h, int kind, float weight_full, float weight_module) {
@@ -499,8 +500,16 @@ int ms_engine_set_loss(void* h, int kind, float weight_full, float weight_module
         for (auto& g : e->graphs) cudaGraphExecDestroy(g.second.exec);       // the loss kernels are baked into the step graphs
         e->graphs.clear();
     }
+    if (kind != e->loss_kind) e->rs_fresh = false;         // proxy_s exists under the proxy loss only
     e->loss_kind = kind; e->proxy_w_full = weight_full; e->proxy_w_module = weight_module;
     return 0;
+}
+size_t ms_engine_reprojection_scratch_floats(void* h, int scale) {
+    size_t n = 0;
+    return static_cast<Engine*>(h)->reprojection_scratch_floats(scale, &n) ? 0 : n;
+}
+int ms_engine_set_reprojection_scale(void* h, int scale, float* scratch, size_t scratch_floats) {
+    return static_cast<Engine*>(h)->set_reprojection_scale(scale, scratch, scratch_floats);
 }
 int ms_engine_forward(void* h, int disp_mask, void* stream) { return static_cast<Engine*>(h)->forward(disp_mask, S(stream)); }
 int ms_engine_loss(void* h, int which, int with_grad, int slot, float grad_scale, void* stream) {

@@ -177,6 +177,21 @@ int resize_bilinear_bwd(const float* dout, int docs, const float* src, int scs, 
                         float* dsrc, int dscs, int rh, int rw, int oh, int ow, float pre_scale, int pre_relu,
                         float post_scale, int post_relu, int accumulate, float* tmp /* B*oh*iw floats */,
                         cudaStream_t st);
+// MAD module losses at 1/s resolution (elementwise.cu).  rs_inputs: legacy bilinear [B,H,W,3] -> [B,h,w,3] of both
+// frames, and proxy [B,H,W] -> [B,h,w] divided by s (proxy and dst_proxy null: no proxy).  rs_module_disp: a module disparity
+// straight from its coarse head, both resizes (to Hp x Wp with the centre crop to H x W, then to h x w) as one separable
+// operator of <= 4 taps per axis built by rs_axis_taps; rs_module_disp_bwd its adjoint, a two-pass gather (deterministic), with
+// the relu mask of the pre-op; tmp holds B*h*iw floats.
+struct RsTap { int i[4]; float w[4]; };
+struct RsRange { int lo, hi; };
+void rs_axis_taps(int in, int r, int o, int n, RsTap* taps /* n */, RsRange* range /* in */);
+int rs_inputs(const float* left, const float* right, const float* proxy, int B, int H, int W, float* dst_left,
+              float* dst_right, float* dst_proxy, int h, int w, int s, cudaStream_t st);
+int rs_module_disp(const float* src, int scs, int B, int ih, int iw, const RsTap* rows, const RsTap* cols, float* dst, int h, int w,
+            float pre_scale, cudaStream_t st);
+int rs_module_disp_bwd(const float* dout, const float* src, int scs, int B, int ih, int iw, const RsTap* rows, const RsRange* rrange,
+                const RsTap* cols, const RsRange* crange, int h, int w, float* dsrc, int dscs, float pre_scale, float* tmp,
+                cudaStream_t st);
 int leaky_bwd(float* g, int gcs, const float* act, int acs, size_t pixels, int c, float alpha, cudaStream_t st);
 int add_channels(float* dst, int dcs, const float* src, int scs, size_t pixels, int c, float scale,
                  int accumulate, cudaStream_t st);

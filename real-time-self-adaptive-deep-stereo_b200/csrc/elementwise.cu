@@ -6,6 +6,9 @@
 //                        relu / x20 / x(-20) scalings of MadNet._make_disp fused in
 //   resize_bilinear_bwd  its transpose (what tf.gradients builds), separable two-pass gather => deterministic
 //   leaky_bwd            gradient of tf.maximum(alpha*x, x)      (Nets/MadNet.py:366-367)
+//   rs_inputs / rs_module_disp / rs_module_disp_bwd
+//                        MAD module losses at 1/s resolution (--reprojectionScale, Stereo_Online_Adaptation.py:22-23,
+//                        91-107; Stereo_Continual_Adaptation.py:95-112)
 #include <algorithm>
 #include "common.cuh"
 
@@ -44,8 +47,8 @@ int pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int Hp
 }
 
 struct Lerp { int i0, i1; float f; };
-__device__ __forceinline__ Lerp lerp_coeff(int o, float scale, int in_size) {
-    // TF 1.x legacy bilinear: src = dst*scale, no half-pixel centres
+__host__ __device__ __forceinline__ Lerp lerp_coeff(int o, float scale, int in_size) {
+    // TF 1.x legacy bilinear: src = dst*scale, no half-pixel centres (on the host: the tap tables of rs_axis_taps)
     float s = (float)o * scale;
     float fl = floorf(s);
     Lerp l;
@@ -186,6 +189,151 @@ int resize_bilinear_bwd(const float* dout, int docs, const float* src, int scs, 
     launch_k(resize_bwd_y_kernel, dim3((unsigned)cdivz(t2, 256)), dim3(256), 0, st, tmp, src, scs, B, ih, iw, dsrc, dscs, rh, oh, ys,
                                                                  pre_scale, pre_relu, accumulate);
     return check_launch("resize_bilinear_bwd", 2);
+}
+
+// ---- MAD module losses at 1/s resolution.  The reference rescales the images with preprocessing.rescale_image (legacy
+// bilinear to (H//s, W//s)) and each module disparity -- already at full resolution, crop(resize(relu(-20 V), Hp x Wp))
+// -- with resize_to_prediction to the same size.
+
+// left_s / right_s (and proxy_s = resize(proxy) / s) of every frame in one pass: one thread per loss-resolution pixel
+__global__ void rs_inputs_kernel(const float* __restrict__ left, const float* __restrict__ right,
+                                 const float* __restrict__ proxy, int B, int H, int W, float* __restrict__ dl,
+                                 float* __restrict__ dr, float* __restrict__ dp, int h, int w, float ys, float xs, float s) {
+    pdl_prologue();
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)B * h * w) return;
+    const int x = (int)(i % w);
+    const size_t q = i / w;
+    const int y = (int)(q % h), b = (int)(q / h);
+    const Lerp ly = lerp_coeff(y, ys, H), lx = lerp_coeff(x, xs, W);
+    const size_t off = (size_t)b * H * W;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        dl[i * 3 + c] = resize_at(left + off * 3 + c, 3, W, ly, lx, 1.f, 0);
+        dr[i * 3 + c] = resize_at(right + off * 3 + c, 3, W, ly, lx, 1.f, 0);
+    }
+    if (dp) dp[i] = resize_at(proxy + off, 1, W, ly, lx, 1.f, 0) / s;      // (a division, as the reference's `/ scale`)
+}
+
+int rs_inputs(const float* left, const float* right, const float* proxy, int B, int H, int W, float* dst_left,
+              float* dst_right, float* dst_proxy, int h, int w, int s, cudaStream_t st) {
+    MS_REQUIRE(B >= 1 && h >= 1 && w >= 1 && h <= H && w <= W && s >= 1, "rs_inputs: bad geometry");
+    MS_REQUIRE(!proxy == !dst_proxy, "rs_inputs: the proxy needs an output and the output a proxy");
+    const size_t total = (size_t)B * h * w;
+    launch_k(rs_inputs_kernel, dim3((unsigned)cdivz(total, 256)), dim3(256), 0, st, left, right, proxy, B, H, W, dst_left,
+             dst_right, dst_proxy, h, w, (float)H / (float)h, (float)W / (float)w, (float)s);
+    return check_launch("rs_inputs");
+}
+
+// One axis of the two resizes as one operator: legacy bilinear in -> r of the pre-op'd source, centre crop to o, legacy
+// bilinear o -> n.  taps[j]: the 4 source indices and weights of output j (a clamped or shared index may repeat);
+// range[i]: the outputs whose taps name source i (lo > hi: none), what the gather of the adjoint walks.
+void rs_axis_taps(int in, int r, int o, int n, RsTap* taps, RsRange* range) {
+    const float s1 = (float)in / (float)r, s2 = (float)o / (float)n;
+    const int c = (r - o) / 2;
+    for (int i = 0; i < in; ++i) range[i] = RsRange{n, -1};
+    for (int j = 0; j < n; ++j) {
+        const Lerp l2 = lerp_coeff(j, s2, o);
+        const int mid[2] = {l2.i0, l2.i1};
+        const double w2[2] = {1.0 - (double)l2.f, (double)l2.f};
+        for (int a = 0; a < 2; ++a) {
+            const Lerp l1 = lerp_coeff(mid[a] + c, s1, in);
+            taps[j].i[2 * a] = l1.i0; taps[j].w[2 * a] = (float)(w2[a] * (1.0 - (double)l1.f));
+            taps[j].i[2 * a + 1] = l1.i1; taps[j].w[2 * a + 1] = (float)(w2[a] * (double)l1.f);
+        }
+        for (int t = 0; t < 4; ++t) {
+            RsRange& g = range[taps[j].i[t]];
+            g.lo = std::min(g.lo, j); g.hi = std::max(g.hi, j);
+        }
+    }
+}
+
+// rs_module_disp: dst[b,y,x] = sum_a rows[y].w[a] * sum_c cols[x].w[c] * relu(pre_scale * src[b, rows[y].i[a], cols[x].i[c]]): both
+// resizes composed in registers, no full-resolution map
+__global__ void rs_disp_kernel(const float* __restrict__ src, int scs, int B, int ih, int iw, const RsTap* __restrict__ rows,
+                               const RsTap* __restrict__ cols, float* __restrict__ dst, int h, int w, float pre_scale) {
+    pdl_prologue();
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)B * h * w) return;
+    const int x = (int)(i % w);
+    const size_t q = i / w;
+    const int y = (int)(q % h), b = (int)(q / h);
+    const float* sb = src + (size_t)b * ih * iw * scs;
+    const RsTap ty = rows[y], tx = cols[x];
+    float acc = 0.f;
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+        const float* sr = sb + (size_t)ty.i[a] * iw * scs;
+        float r = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) r += tx.w[c] * pre_op(sr[(size_t)tx.i[c] * scs], pre_scale, 1);
+        acc += ty.w[a] * r;
+    }
+    dst[i] = acc;
+}
+
+int rs_module_disp(const float* src, int scs, int B, int ih, int iw, const RsTap* rows, const RsTap* cols, float* dst, int h, int w,
+            float pre_scale, cudaStream_t st) {
+    MS_REQUIRE(rows && cols && B >= 1 && h >= 1 && w >= 1, "rs_module_disp: bad arguments");
+    const size_t total = (size_t)B * h * w;
+    launch_k(rs_disp_kernel, dim3((unsigned)cdivz(total, 256)), dim3(256), 0, st, src, scs, B, ih, iw, rows, cols, dst, h, w,
+             pre_scale);
+    return check_launch("rs_module_disp");
+}
+
+// adjoint of rs_module_disp, x pass: tmp[b,y,ix] = sum over the outputs x that name ix of dout[b,y,x] * (its weights on ix)
+__global__ void rs_disp_bwd_x_kernel(const float* __restrict__ dout, const RsTap* __restrict__ cols,
+                                     const RsRange* __restrict__ crange, int B, int h, int w, int iw, float* __restrict__ tmp) {
+    pdl_prologue();
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)B * h * iw) return;
+    const int ix = (int)(i % iw);
+    const float* g = dout + (i / iw) * w;
+    const RsRange rg = crange[ix];
+    float acc = 0.f;
+    for (int x = rg.lo; x <= rg.hi; ++x) {
+        const RsTap t = cols[x];
+        float wgt = 0.f;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) if (t.i[c] == ix) wgt += t.w[c];
+        acc += g[x] * wgt;
+    }
+    tmp[i] = acc;
+}
+
+// y pass: dsrc[b,iy,ix] = relu'(pre_scale * src) * pre_scale * sum over the outputs y that name iy of tmp * (weights)
+__global__ void rs_disp_bwd_y_kernel(const float* __restrict__ tmp, const RsTap* __restrict__ rows,
+                                     const RsRange* __restrict__ rrange, const float* __restrict__ src, int scs, int B, int ih,
+                                     int iw, int h, float* __restrict__ dsrc, int dscs, float pre_scale) {
+    pdl_prologue();
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)B * ih * iw) return;
+    const int ix = (int)(i % iw);
+    const size_t q = i / iw;
+    const int iy = (int)(q % ih), b = (int)(q / ih);
+    const RsRange rg = rrange[iy];
+    float acc = 0.f;
+    for (int y = rg.lo; y <= rg.hi; ++y) {
+        const RsTap t = rows[y];
+        float wgt = 0.f;
+#pragma unroll
+        for (int a = 0; a < 4; ++a) if (t.i[a] == iy) wgt += t.w[a];
+        acc += tmp[((size_t)b * h + y) * iw + ix] * wgt;
+    }
+    const float d = src[i * scs] * pre_scale > 0.f ? pre_scale : 0.f;
+    dsrc[i * dscs] = acc * d;
+}
+
+int rs_module_disp_bwd(const float* dout, const float* src, int scs, int B, int ih, int iw, const RsTap* rows, const RsRange* rrange,
+                const RsTap* cols, const RsRange* crange, int h, int w, float* dsrc, int dscs, float pre_scale, float* tmp,
+                cudaStream_t st) {
+    MS_REQUIRE(rows && rrange && cols && crange && tmp && B >= 1 && h >= 1 && w >= 1, "rs_module_disp_bwd: bad arguments");
+    const size_t t1 = (size_t)B * h * iw;
+    launch_k(rs_disp_bwd_x_kernel, dim3((unsigned)cdivz(t1, 256)), dim3(256), 0, st, dout, cols, crange, B, h, w, iw, tmp);
+    const size_t t2 = (size_t)B * ih * iw;
+    launch_k(rs_disp_bwd_y_kernel, dim3((unsigned)cdivz(t2, 256)), dim3(256), 0, st, tmp, rows, rrange, src, scs, B, ih, iw, h,
+             dsrc, dscs, pre_scale);
+    return check_launch("rs_module_disp_bwd", 2);
 }
 
 __global__ void leaky_bwd_kernel(float* __restrict__ g, int gcs, const float* __restrict__ act, int acs,

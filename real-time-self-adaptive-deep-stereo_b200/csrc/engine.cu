@@ -48,6 +48,7 @@ Engine::Engine()
     dp_rank = 0; dp_world = 1; dp_connected = false; dp_xbuf = nullptr; dp_state = nullptr; dp_cap_floats = 0;
     opt_kind = 0; adam_b1 = adam_b2 = adam_eps = 0.f; adam_v = nullptr; adam_powers = nullptr;
     rect_map_l = rect_map_r = nullptr; rect_h = rect_w = 0; rect_scratch = nullptr;
+    rs_scale = 1; rs_fresh = false; memset(rs_tab, 0, sizeof rs_tab);
 }
 
 void Engine::drop_graphs() {
@@ -567,6 +568,7 @@ int Engine::set_input(const float* left, const float* right, cudaStream_t st) {
     size_t bytes = (size_t)B * H * W * 3 * sizeof(float);
     MS_CHECK_CUDA(cudaMemcpyAsync(rl.p, left, bytes, cudaMemcpyDefault, st));
     MS_CHECK_CUDA(cudaMemcpyAsync(rr.p, right, bytes, cudaMemcpyDefault, st));
+    rs_fresh = false;
     return 0;
 }
 
@@ -579,6 +581,7 @@ int Engine::set_input_u8(const unsigned char* left, const unsigned char* right, 
     unsigned char* right_stage = u8_stage + u8_stage_right_offset(n);
     MS_CHECK_CUDA(cudaMemcpyAsync(u8_stage, left, n, cudaMemcpyDefault, st));
     MS_CHECK_CUDA(cudaMemcpyAsync(right_stage, right, n, cudaMemcpyDefault, st));
+    rs_fresh = false;
     if (u8_to_f32(u8_stage, rl.p, n, st)) return -1;
     return u8_to_f32(right_stage, rr.p, n, st);
 }
@@ -588,6 +591,7 @@ int Engine::set_input_u8(const unsigned char* left, const unsigned char* right, 
 int Engine::set_input_u8_resized(const unsigned char* left, const unsigned char* right, int h, int w, int rh, int rw,
                                  cudaStream_t st) {
     MS_REQUIRE(bound, "engine not bound");
+    rs_fresh = false;
     if (rect_map_l) {
         MS_REQUIRE(h == rect_h && w == rect_w, "set_input_u8_resized: frames are " + std::to_string(h) + "x" + std::to_string(w) +
                                                ", the rectification tables " + std::to_string(rect_h) + "x" + std::to_string(rect_w));
@@ -613,6 +617,82 @@ int Engine::set_rectification(const float* map_left, const float* map_right, int
     MS_REQUIRE(scratch && scratch_bytes >= need,
                "set_rectification: the scratch must hold both rectified frames (" + std::to_string(need) + " bytes)");
     rect_map_l = map_left; rect_map_r = map_right; rect_h = h; rect_w = w; rect_scratch = scratch;
+    return 0;
+}
+
+// The scratch of module losses at 1/s resolution: left_s, right_s, proxy_s, the module disparity at loss resolution, then
+// per module (source V[6-g], or final_ for module 4) the tap tables of rs_disp.  base == nullptr: sizing only.
+size_t Engine::rs_layout(int s, float* base) {
+    Bump A{base ? base : reinterpret_cast<float*>(uintptr_t{256}), 0};
+    const int h = H / s, w = W / s;
+    TView l = A.tens(B, h, w, 3), r = A.tens(B, h, w, 3), p = A.tens(B, h, w, 1), d = A.tens(B, h, w, 1);
+    RsTables t[5];
+    for (int g = 0; g < 5; ++g) {
+        const TView& src = g < 4 ? V[6 - g] : final_;
+        t[g].rows = reinterpret_cast<RsTap*>(A.alloc((size_t)h * sizeof(RsTap) / sizeof(float)));
+        t[g].cols = reinterpret_cast<RsTap*>(A.alloc((size_t)w * sizeof(RsTap) / sizeof(float)));
+        t[g].rrange = reinterpret_cast<RsRange*>(A.alloc((size_t)src.h * sizeof(RsRange) / sizeof(float)));
+        t[g].crange = reinterpret_cast<RsRange*>(A.alloc((size_t)src.w * sizeof(RsRange) / sizeof(float)));
+    }
+    if (base) {
+        rs_left = l; rs_right = r; rs_proxy = p; rs_disp = d;
+        for (int g = 0; g < 5; ++g) rs_tab[g] = t[g];
+    }
+    return A.off;
+}
+
+int Engine::reprojection_scratch_floats(int s, size_t* floats) {
+    *floats = 0;
+    MS_REQUIRE(s >= 1, "reprojection scale must be >= 1, got " + std::to_string(s));
+    if (s == 1) return 0;
+    // the reference asserts one train op per side output, which DispNet does not have (Stereo_Online_Adaptation.py:97)
+    MS_REQUIRE(net == 0, "reprojection scale " + std::to_string(s) + ": only MADNet has MAD train ops (DispNet: scale 1)");
+    MS_REQUIRE(bound, "reprojection scale: engine not bound");
+    MS_REQUIRE(H / s >= 3 && W / s >= 3, "reprojection scale " + std::to_string(s) + ": the loss resolution " +
+                                         std::to_string(H / s) + "x" + std::to_string(W / s) + " is below the 3x3 SSIM window");
+    *floats = rs_layout(s, nullptr);
+    return 0;
+}
+
+int Engine::set_reprojection_scale(int s, float* scratch, size_t scratch_floats) {
+    size_t need = 0;
+    if (s == 1 || (s > 1 && !scratch)) {        // back to full-resolution module losses
+        if (rs_scale != 1) drop_graphs();
+        rs_scale = 1; rs_fresh = false;
+        for (const char* n : {"rs_left", "rs_right", "rs_proxy", "rs_disp"}) tensors.erase(n);
+        return 0;
+    }
+    if (reprojection_scratch_floats(s, &need)) return -2;
+    MS_REQUIRE(scratch_floats >= need, "set_reprojection_scale: the scratch holds " + std::to_string(scratch_floats) +
+                                       " floats, scale " + std::to_string(s) + " needs " + std::to_string(need));
+    MS_REQUIRE((reinterpret_cast<uintptr_t>(scratch) & 15) == 0, "set_reprojection_scale: the scratch must be 16B aligned");
+    const int h = H / s, w = W / s;
+    std::vector<RsTap> rows(h), cols(w);
+    std::vector<RsRange> rr, cr;
+    MS_CHECK_CUDA(cudaDeviceSynchronize());     // a step in flight may still read the tables being replaced
+    rs_layout(s, scratch);
+    for (int g = 0; g < 5; ++g) {
+        const TView& src = g < 4 ? V[6 - g] : final_;
+        rr.resize(src.h); cr.resize(src.w);
+        rs_axis_taps(src.h, Hp, H, h, rows.data(), rr.data());
+        rs_axis_taps(src.w, Wp, W, w, cols.data(), cr.data());
+        MS_CHECK_CUDA(cudaMemcpy(rs_tab[g].rows, rows.data(), rows.size() * sizeof(RsTap), cudaMemcpyHostToDevice));
+        MS_CHECK_CUDA(cudaMemcpy(rs_tab[g].cols, cols.data(), cols.size() * sizeof(RsTap), cudaMemcpyHostToDevice));
+        MS_CHECK_CUDA(cudaMemcpy(rs_tab[g].rrange, rr.data(), rr.size() * sizeof(RsRange), cudaMemcpyHostToDevice));
+        MS_CHECK_CUDA(cudaMemcpy(rs_tab[g].crange, cr.data(), cr.size() * sizeof(RsRange), cudaMemcpyHostToDevice));
+    }
+    drop_graphs();                              // the loss-resolution kernels and buffers are baked into the step graphs
+    rs_scale = s; rs_fresh = false;
+    tensors["rs_left"] = rs_left; tensors["rs_right"] = rs_right; tensors["rs_proxy"] = rs_proxy; tensors["rs_disp"] = rs_disp;
+    return 0;
+}
+
+// left_s, right_s (and proxy_s under the proxy loss) of the current frame
+int Engine::rs_prepare_inputs(cudaStream_t st) {
+    const bool px = loss_kind == 1;
+    if (rs_inputs(tensors["raw_left"].p, tensors["raw_right"].p, px ? proxy : nullptr, B, H, W, rs_left.p, rs_right.p,
+                  px ? rs_proxy.p : nullptr, rs_left.h, rs_left.w, rs_scale, st)) return -1;
+    rs_fresh = true;
     return 0;
 }
 
@@ -711,6 +791,28 @@ int Engine::loss(int which, int with_grad, int slot, float grad_scale, cudaStrea
     MS_REQUIRE(bound && which >= 0 && which < n_disp && slot >= 0 && slot < 2, "loss: bad arguments");
     // the full-resolution loss of a MAD step runs beside the module's loss (mad_branch): a workspace of its own
     float* ws = slot == 0 && !with_grad && loss_full_ws ? loss_full_ws : loss_ws;
+    if (rs_module(which, slot)) {
+        // Stereo_Online_Adaptation.py:91-107 / Stereo_Continual_Adaptation.py:95-112 at scale s: the module disparity and
+        // the images (proxy) at H/s x W/s.  The reference's multiplier H // p.shape[1] is 1 (its disparities are already
+        // full resolution), so the disparity stays in full-resolution pixels: kept as the reference computes it
+        if (!rs_fresh && rs_prepare_inputs(st)) return -1;
+        const TView& src = which < 4 ? V[6 - which] : final_;
+        const int h = rs_disp.h, w = rs_disp.w;
+        prof_begin(CAT_LOSS, st);
+        int rc = rs_module_disp(src.p, src.cs, B, src.h, src.w, rs_tab[which].rows, rs_tab[which].cols, rs_disp.p, h, w, -20.f, st);
+        if (!rc && loss_kind == 1) {
+            rc = proxy_loss(rs_disp.p, rs_proxy.p, B * h * w, proxy_w_module, grad_scale, scalars + slot,
+                            with_grad ? g_disp.p : nullptr, ws, st);
+        } else if (!rc) {
+            ReprojLoss p{};
+            p.left = rs_left.p; p.right = rs_right.p; p.disp = rs_disp.p; p.loss = scalars + slot;
+            p.ddisp = with_grad ? g_disp.p : nullptr;
+            p.workspace = ws; p.B = B; p.H = h; p.W = w; p.grad_scale = grad_scale;
+            rc = reproj_loss(p, st);
+        }
+        prof_end(st);
+        return rc;
+    }
     if (loss_kind == 1) {
         // Stereo_Continual_Adaptation.py:75 (full-resolution loss, weight 0.01; also the FULL train op :133) and :112
         // (module losses, weight 0.1)
@@ -873,8 +975,12 @@ int Engine::backward_impl(int mode, int group, cudaStream_t st) {
         const bool need_feat = lo_pyr <= f;
         const TView& head = (k == 2) ? final_ : V[k];
         TView& ghead = (k == 2) ? g_final : g_V[k];
-        if (resize_bilinear_bwd(g_disp.p, 1, head.p, head.cs, B, head.h, head.w, ghead.p, 1, Hp, Wp, H, W, -20.f, 1,
-                                1.f, 0, 0, rs_tmp, st)) return -1;
+        if (rs_scale > 1) {     // the module loss ran at 1/s resolution (loss): its gradient [B,h,w] is in g_disp
+            const RsTables& t = rs_tab[group];
+            if (rs_module_disp_bwd(g_disp.p, head.p, head.cs, B, head.h, head.w, t.rows, t.rrange, t.cols, t.crange, rs_disp.h,
+                            rs_disp.w, ghead.p, 1, -20.f, rs_tmp, st)) return -1;
+        } else if (resize_bilinear_bwd(g_disp.p, 1, head.p, head.cs, B, head.h, head.w, ghead.p, 1, Hp, Wp, H, W, -20.f, 1,
+                                       1.f, 0, 0, rs_tmp, st)) return -1;
         if (k == 2) {
             bool est_train = any_trainable(est_layer(2, 1), est_layer(2, 6));
             if (ctx_bwd(need_feat || est_train)) return -1;
@@ -938,7 +1044,8 @@ int Engine::run_eager(int mode, int group, int disp_mask, int with_update, float
                       cudaStream_t st) {
     const int full = n_disp - 1;
     int mask = disp_mask | (1 << full);
-    if (mode == 1) mask |= 1 << group;
+    const bool rs = mode == 1 && rs_scale > 1 && net == 0;     // module loss at 1/s: read straight from the coarse head
+    if (mode == 1 && !rs) mask |= 1 << group;
     // NVTX ranges (SURVEY section 5: tracing): visible in nsys / ncu timelines, free when no tool is attached
     struct Range { explicit Range(const char* n) { nvtxRangePushA(n); } ~Range() { nvtxRangePop(); } };
     const bool branch = mad_branch(mode, group);
@@ -948,6 +1055,18 @@ int Engine::run_eager(int mode, int group, int disp_mask, int with_update, float
         MS_CHECK_CUDA(cudaEventCreateWithFlags(&ev_bjoin, cudaEventDisableTiming));
     }
     cudaStream_t bs = branch ? bstream : st;     // the train op's stream
+    if (rs) {       // the loss-resolution images only need the input: on the train op's stream, beside the forward
+        Range r("madstereo/loss_inputs");
+        if (branch) {
+            MS_CHECK_CUDA(cudaEventRecord(ev_bfork, st));
+            MS_CHECK_CUDA(cudaStreamWaitEvent(bs, ev_bfork, 0));
+        }
+        const bool pdl = pdl_enabled();
+        if (branch) pdl_set_suppressed(true);
+        const int rc = rs_prepare_inputs(bs);
+        pdl_set_suppressed(!pdl);
+        if (rc) return rc;
+    }
     { Range r("madstereo/forward"); if (forward(mask, st, branch ? group : -1, branch ? bstream : nullptr)) return -1; }
     { Range r("madstereo/loss_full"); if (loss(full, mode == 2, 0, 1.f, st)) return -1; }
     if (mode == 1) {
@@ -1030,6 +1149,7 @@ int Engine::run(int mode, int group, int disp_mask, int with_update, float lr, f
     MS_CHECK_CUDA(cudaStreamWaitEvent(gstream, ev_in, 0));
     MS_CHECK_CUDA(cudaGraphLaunch(it->second.exec, gstream));
     add_launches(it->second.kernels);
+    if (mode == 1 && rs_scale > 1) rs_fresh = true;     // the step wrote this frame's loss-resolution inputs
     MS_CHECK_CUDA(cudaEventRecord(ev_out, gstream));
     MS_CHECK_CUDA(cudaStreamWaitEvent(st, ev_out, 0));
     if (profiling == 2 && it->second.spans) {        // in-graph timing: read the event nodes of THIS replay

@@ -151,6 +151,20 @@ struct Engine {
     const float* rect_map_l; const float* rect_map_r;
     int rect_h, rect_w;
     unsigned char* rect_scratch;
+    // MAD module losses at 1/rs_scale resolution (ms_engine_set_reprojection_scale, --reprojectionScale); rs_scale 1: full
+    // resolution.  Views and tap tables live in the caller's scratch: rs_left / rs_right [B,h,w,3], rs_proxy / rs_disp
+    // [B,h,w,1] (h = H / rs_scale, w = W / rs_scale); per module the row / column taps of rs_module_disp and their ranges.  The
+    // module loss's gradient [B,h,w] reuses g_disp.  rs_fresh: rs_left / rs_right / rs_proxy hold the current frame's values
+    int rs_scale;
+    TView rs_left, rs_right, rs_proxy, rs_disp;
+    struct RsTables { RsTap *rows, *cols; RsRange *rrange, *crange; };
+    RsTables rs_tab[5];
+    bool rs_fresh;
+    size_t rs_layout(int s, float* base);          // scratch floats; base != nullptr: also place the views and tables
+    int reprojection_scratch_floats(int s, size_t* floats);
+    int set_reprojection_scale(int s, float* scratch, size_t scratch_floats);
+    bool rs_module(int which, int slot) const { return rs_scale > 1 && net == 0 && slot == 1 && which >= 0 && which < 5; }
+    int rs_prepare_inputs(cudaStream_t st);
     // optimizer of update(): 0 = momentum SGD (Mo = accumulator), 1 = Adam (Mo = first moment, adam_v = second moment,
     // adam_powers = device [beta1_power, beta2_power] shared by every train op); caller-owned storage (ms_engine_set_optimizer)
     int opt_kind;

@@ -77,6 +77,8 @@ _SIGS = {
     'ms_engine_set_gt': (I, [P, P, P]),
     'ms_engine_set_proxy': (I, [P, P, P]),
     'ms_engine_set_loss': (I, [P, I, F, F]),
+    'ms_engine_reprojection_scratch_floats': (Z, [P, I]),
+    'ms_engine_set_reprojection_scale': (I, [P, I, P, Z]),
     'ms_engine_dp_create': (I, [P, I, I, P]),
     'ms_engine_dp_connect': (I, [P, P]),
     'ms_engine_dp_error': (I, [P, P]),

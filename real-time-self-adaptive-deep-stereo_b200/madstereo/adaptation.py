@@ -46,12 +46,14 @@ class OnlineAdaptation(object):
     def __init__(self, net, mode='MAD', train_config=None, lr=0.0001, momentum=0.9, sample_mode='SEQUENTIAL',
                  num_blocks=1, fixed_id=0, sample_frequency=1, ssim_th=0.5, process_group=None,
                  loss='reprojection', decay=0.99, uf=0.01, dilation=1, optimizer='momentum', beta1=0.9, beta2=0.999,
-                 epsilon=1e-8):
+                 epsilon=1e-8, reprojection_scale=1):
         """loss='proxy', decay, uf, dilation: the continual-adaptation variant (Stereo_Continual_Adaptation.py): masked L1 to
         proxy disparities (weights 0.01 full-resolution / FULL, 0.1 per MAD module, :75,112), reward recurrence
         h <- decay*h, h[i] += uf*gain (:232-234), a train op only every `dilation`-th frame (:212).
         optimizer='adam': tf.train.AdamOptimizer(lr) with TF1's defaults, as the live demo adapts (Demo/demo_model.py:163);
-        one pair of bias-correction powers shared by every train op.  Single GPU only."""
+        one pair of bias-correction powers shared by every train op.  Single GPU only.
+        reprojection_scale: the MAD module losses at 1/reprojection_scale resolution (--reprojectionScale,
+        Stereo_Online_Adaptation.py:91-107); no effect under FULL / NONE, as in the reference.  MADNet only."""
         assert mode in ('NONE', 'FULL', 'MAD')
         assert loss in ('reprojection', 'proxy')
         assert optimizer in ('momentum', 'adam')
@@ -89,6 +91,10 @@ class OnlineAdaptation(object):
             self.engine.set_loss('proxy')
         if optimizer == 'adam':
             self.engine.set_optimizer('adam', beta1, beta2, epsilon)
+        if int(reprojection_scale) < 1:
+            raise MadStereoError('reprojection_scale must be >= 1, got %r' % (reprojection_scale,))
+        if mode == 'MAD' and int(reprojection_scale) != 1:
+            self.engine.set_reprojection_scale(reprojection_scale)
         self._adam_snapshot = None
         self.num_actions = len(self.groups) if mode == 'MAD' else (1 if mode == 'FULL' else 0)
         self.fetch_counter = [0] * self.num_actions

@@ -67,6 +67,8 @@ class StereoEngine:
         self.resize_shape = None      # set_resize(): None = uint8 frames must be [B,H,W,3]; else (rh, rw), -1 = no rescale
         self._rs_stage = None
         self._rect = None             # set_rectification(): (left table, right table, scratch) the engine reads per frame
+        self.reprojection_scale = 1
+        self._rs_scratch = None       # set_reprojection_scale(): the loss-resolution buffers and tap tables
 
     def _on_device(self):
         """Context that makes this engine's GPU current -- a no-op object when it already is (the per-frame calls of a
@@ -292,6 +294,26 @@ class StereoEngine:
         k = {'reprojection': 0, 'proxy': 1}[kind]
         check(self._lib.ms_engine_set_loss(self._h, k, weight_full, weight_module), 'set_loss')
 
+    def set_reprojection_scale(self, scale):
+        """Compute the MAD module losses at 1/scale resolution, as the reference's --reprojectionScale does: frames (or the
+        proxy, divided by scale) and the module disparity resized to (H // scale, W // scale).  The disparity keeps its
+        full-resolution units there, as in the reference.  The full-resolution loss, FULL and NONE are unchanged.  1 turns
+        it off.  MADNet only; needs bind().  Changing the scale drops the captured step graphs."""
+        scale = int(scale)
+        if not self.bound:
+            raise MadStereoError('set_reprojection_scale: bind() first')
+        if scale == 1:
+            check(self._lib.ms_engine_set_reprojection_scale(self._h, 1, c_void_p(0), 0), 'set_reprojection_scale')
+            self.reprojection_scale, self._rs_scratch = 1, None
+            return
+        n = self._lib.ms_engine_reprojection_scratch_floats(self._h, scale)
+        if n == 0:
+            raise MadStereoError('set_reprojection_scale: %s' % self._lib.ms_last_error().decode())
+        scratch = torch.empty(n, dtype=torch.float32, device=self.device)
+        with self._on_device():
+            check(self._lib.ms_engine_set_reprojection_scale(self._h, scale, _ptr(scratch), n), 'set_reprojection_scale')
+        self.reprojection_scale, self._rs_scratch = scale, scratch
+
     def _as_f32(self, x, c=3):
         if isinstance(x, np.ndarray):
             x = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
@@ -409,5 +431,8 @@ class StereoEngine:
     def tensor(self, name):
         """torch view [n,h,w,c] (strided) of an engine tensor inside the workspace."""
         p, (n, h, w, c, cs) = self.tensor_info(name)
-        off = (p - self.workspace.data_ptr()) // 4
-        return self.workspace.as_strided((n, h, w, c), (h * w * cs, w * cs, cs, 1), off)
+        base = self.workspace
+        if self._rs_scratch is not None and 0 <= p - self._rs_scratch.data_ptr() < 4 * self._rs_scratch.numel():
+            base = self._rs_scratch                   # rs_left / rs_right / rs_proxy / rs_disp
+        off = (p - base.data_ptr()) // 4
+        return base.as_strided((n, h, w, c), (h * w * cs, w * cs, cs, 1), off)

@@ -9,7 +9,10 @@ min(t(MAD g) - t(NONE), the forward after module g's disparity exists).  The sec
 instrumented NONE replay (event nodes inside the step graph): the forward convolutions after the head conv of the
 module's level (module 4: none), the correlations of the later levels and the full-resolution loss.
 
-    python tools/step_phases.py [--replays 300] [--rounds 3] [--height 384] [--width 1280]
+--reprojection-scale 1 2 4 also times every MAD module with its loss at 1/2 and 1/4 resolution (`MAD<g>_s<s>`), each
+scale on an engine of its own, interleaved with the rest.
+
+    python tools/step_phases.py [--replays 300] [--rounds 3] [--height 384] [--width 1280] [--reprojection-scale 1 ...]
 """
 import argparse
 import json
@@ -43,7 +46,11 @@ def main():
     ap.add_argument('--rounds', type=int, default=3)
     ap.add_argument('--height', type=int, default=384)
     ap.add_argument('--width', type=int, default=1280)
+    ap.add_argument('--reprojection-scale', type=int, nargs='+', default=[1],
+                    help='MAD module losses at 1/s resolution; 1 (the NONE / FULL / MAD<g> modes) must be among them')
     a = ap.parse_args()
+    if 1 not in a.reprojection_scale:
+        ap.error('--reprojection-scale: include 1')
     import Nets
     from madstereo.adaptation import OnlineAdaptation
     from madstereo.engine import MODE_FULL, MODE_MAD, MODE_NONE
@@ -58,24 +65,35 @@ def main():
                                              radius_d=2, stride=1, is_training=False))
     cfg = json.load(open(os.path.join(PKG, 'block_config', 'MadNet_full.json')))
     ad = OnlineAdaptation(net, mode='MAD', train_config=cfg, lr=1e-4, sample_mode='SEQUENTIAL')
-    sys.stdout = real_stdout
     eng = net.engine
     ad.load_weights(init_params(eng.layers, seed=42))
     eng.set_input(lt, rt)
+    scaled = {}                                    # scale -> an engine whose MAD module losses run at 1/scale
+    for sc in sorted(set(a.reprojection_scale) - {1}):
+        n2 = Nets.get_stereo_net('MADNet', dict(left_img=lt, right_img=rt, split_layers=[None], sequence=True,
+                                                train_portion='BEGIN', bulkhead=True, warping=True, context_net=True,
+                                                radius_d=2, stride=1, is_training=False))
+        ad2 = OnlineAdaptation(n2, mode='MAD', train_config=cfg, lr=1e-4, sample_mode='SEQUENTIAL', reprojection_scale=sc)
+        ad2.load_weights(init_params(n2.engine.layers, seed=42))
+        n2.engine.set_input(lt, rt)
+        scaled[sc] = n2.engine
+    sys.stdout = real_stdout
 
-    modes = [('NONE', MODE_NONE, 0)] + [('MAD%d' % g, MODE_MAD, g) for g in range(eng.n_groups)] + [('FULL', MODE_FULL, 0)]
-    run = lambda m, g: eng.run(m, g, 0, m != MODE_NONE, 1e-4, 0.9, 1.0)
-    for _, m, g in modes:                          # capture + warm-up
+    modes = [('NONE', MODE_NONE, 0, eng)] + [('MAD%d' % g, MODE_MAD, g, eng) for g in range(eng.n_groups)] + \
+        [('FULL', MODE_FULL, 0, eng)] + [('MAD%d_s%d' % (g, sc), MODE_MAD, g, e) for sc, e in scaled.items()
+                                         for g in range(e.n_groups)]
+    run = lambda m, g, e=eng: e.run(m, g, 0, m != MODE_NONE, 1e-4, 0.9, 1.0)
+    for _, m, g, e in modes:                       # capture + warm-up
         for _ in range(5):
-            run(m, g)
+            run(m, g, e)
     torch.cuda.synchronize()
-    times = {name: [] for name, _, _ in modes}
+    times = {name: [] for name, _, _, _ in modes}
     for _ in range(a.rounds):
-        for name, m, g in modes:
+        for name, m, g, e in modes:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(a.replays):
-                run(m, g)
+                run(m, g, e)
             e1.record()
             e1.synchronize()
             times[name].append(1e3 * e0.elapsed_time(e1) / a.replays)
