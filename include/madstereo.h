@@ -304,6 +304,11 @@ int ms_engine_num_tensors(void* e);
 int ms_engine_tensor_name(void* e, int i, char* name, int cap);
 /* dims: n,h,w,c,cs */
 int ms_engine_tensor(void* e, const char* name, float** ptr, int* dims5);
+/* Read-only view of layer i's plan, valid after ms_engine_bind: kinds = the kernels of its forward, input gradient and
+ * weight gradient (engine.h ConvPlan: Fwd HEAD 0, ONE_CHANNEL 1, STEM 2, SMALL 3, BF 4, GEMM 5; Dgrad HEAD 0, BF 1,
+ * GEMM 2; Wgrad BF 0, STEM 1, HEAD 2, FP32 3); ptrs / dims = its views x, y, dpre, dx, each {n,h,w,c,cs} (dims is 4 x 5).
+ * The input gradient dx is written only when the layer has one: ptrs[3] == NULL means none. */
+int ms_engine_layer_plan(void* e, int i, int* kinds3, float** ptrs4, int* dims20);
 
 #ifdef __cplusplus
 }

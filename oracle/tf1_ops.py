@@ -10,7 +10,7 @@ TensorFlow's own kernels.
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
 import this package.  The product path (real-time-self-adaptive-deep-stereo_b200/) never does.
 
-All tensors are NHWC torch CPU tensors (fp32 by default, fp64 for cross-checks); conv kernels are
+All tensors are NHWC torch tensors on any device (fp32 by default, fp64 for cross-checks); conv kernels are
 HWIO [kh,kw,cin,cout] exactly like the reference's tf.get_variable shapes.
 """
 import math
@@ -111,7 +111,7 @@ def crop_or_pad(x, th, tw):
     return x
 
 
-def _resize_axis_coeffs(in_size, out_size, dtype):
+def _resize_axis_coeffs(in_size, out_size, dtype, device=None):
     # TF 1.x legacy bilinear (align_corners=False, no half-pixel centres):
     # scale = in/out (float32); src = dst*scale; lo=floor(src); hi=min(lo+1,in-1); lerp=src-lo
     scale = torch.tensor(in_size / out_size, dtype=torch.float32)
@@ -120,7 +120,7 @@ def _resize_axis_coeffs(in_size, out_size, dtype):
     lo = torch.floor(src)
     hi = torch.clamp(lo + 1, max=in_size - 1)
     lerp = (src - lo).to(dtype)
-    return lo.long(), hi.long(), lerp
+    return lo.long().to(device), hi.long().to(device), lerp.to(device)
 
 
 def resize_bilinear(x, oh, ow):
@@ -131,8 +131,8 @@ def resize_bilinear(x, oh, ow):
     h, w = x.shape[1], x.shape[2]
     if h == oh and w == ow:
         return x
-    ylo, yhi, yl = _resize_axis_coeffs(h, oh, x.dtype)
-    xlo, xhi, xl = _resize_axis_coeffs(w, ow, x.dtype)
+    ylo, yhi, yl = _resize_axis_coeffs(h, oh, x.dtype, x.device)
+    xlo, xhi, xl = _resize_axis_coeffs(w, ow, x.dtype, x.device)
     top = x[:, ylo]
     bot = x[:, yhi]
     xl = xl.view(1, 1, -1, 1)
@@ -165,7 +165,7 @@ def linear_warp(feat, u):
     Taps falling outside [0,w-1] get weight 0 (weights masked, indices clamped).
     """
     b, h, w, c = feat.shape
-    xs = torch.arange(w, dtype=feat.dtype).view(1, 1, w, 1)
+    xs = torch.arange(w, dtype=feat.dtype, device=feat.device).view(1, 1, w, 1)
     cx = xs + u
     x0 = torch.floor(cx)
     x1 = x0 + 1
@@ -187,7 +187,7 @@ def warp_image(img, disp):
     wt_y1 == 0 and only the row itself contributes.
     """
     b, h, w, c = img.shape
-    xs = torch.arange(w, dtype=img.dtype).view(1, 1, w, 1)
+    xs = torch.arange(w, dtype=img.dtype, device=img.device).view(1, 1, w, 1)
     cx = xs - disp
     x0 = torch.floor(cx)
     x1 = x0 + 1

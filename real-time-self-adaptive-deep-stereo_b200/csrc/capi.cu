@@ -593,5 +593,18 @@ int ms_engine_tensor(void* h, const char* name, float** ptr, int* dims5) {
     if (dims5) { dims5[0] = it->second.n; dims5[1] = it->second.h; dims5[2] = it->second.w; dims5[3] = it->second.c; dims5[4] = it->second.cs; }
     return 0;
 }
+int ms_engine_layer_plan(void* h, int i, int* kinds3, float** ptrs4, int* dims20) {
+    Engine* e = static_cast<Engine*>(h);
+    if (!e->bound) { set_error("ms_engine_layer_plan: engine not bound"); return -2; }
+    if (i < 0 || i >= (int)e->plan.size()) { set_error("layer index out of range"); return -2; }
+    const ConvPlan& P = e->plan[i];
+    if (kinds3) { kinds3[0] = P.fwd; kinds3[1] = P.dgrad; kinds3[2] = P.wgrad; }
+    const TView* v[4] = {&P.x, &P.y, &P.dpre, &P.dx};
+    for (int k = 0; k < 4; ++k) {
+        if (ptrs4) ptrs4[k] = v[k]->p;
+        if (dims20) { int* d = dims20 + 5 * k; d[0] = v[k]->n; d[1] = v[k]->h; d[2] = v[k]->w; d[3] = v[k]->c; d[4] = v[k]->cs; }
+    }
+    return 0;
+}
 
 }  // extern "C"

@@ -90,11 +90,13 @@ void Engine::layout_dispnet(Bump& A) {
         tensors[n + "/up_predict"] = slice(d_cat[u], S.skip + S.cout, 1);
         tensors[n + "/concat"] = d_cc[u];
         tensors["grad/" + n + "/concat"] = gd_cc[u];
+        tensors[n + "/cat"] = d_cat[u]; tensors["grad/" + n + "/cat"] = gd_cat[u];    // [skip | deconv | up_predict]
+        tensors["grad/" + n + "/predict"] = gd_pr[u];
         bh *= 2; bw *= 2;
     }
     d_pred = A.tens(B, h2, w2, 1); gd_pred = A.tens(B, h2, w2, 1);
     plan_views(DN_PRED, d_cc[4], d_pred, gd_pred, gd_cc[4]);
-    tensors["prediction"] = d_pred;
+    tensors["prediction"] = d_pred; tensors["grad/prediction"] = gd_pred;
 }
 
 int Engine::forward_dispnet(int disp_mask, cudaStream_t st) {

@@ -98,6 +98,7 @@ _SIGS = {
     'ms_engine_num_tensors': (I, [P]),
     'ms_engine_tensor_name': (I, [P, I, c_char_p, I]),
     'ms_engine_tensor': (I, [P, c_char_p, POINTER(P), POINTER(I)]),
+    'ms_engine_layer_plan': (I, [P, I, POINTER(I), POINTER(P), POINTER(I)]),
 }
 
 EXPORTS = sorted(_SIGS)

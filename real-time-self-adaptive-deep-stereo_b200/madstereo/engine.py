@@ -428,9 +428,28 @@ class StereoEngine:
         check(self._lib.ms_engine_tensor(self._h, name.encode(), byref(p), dims), 'tensor')
         return p.value, tuple(dims)
 
+    FWD_KINDS = ('HEAD', 'ONE_CHANNEL', 'STEM', 'SMALL', 'BF', 'GEMM')
+    DGRAD_KINDS = ('HEAD', 'BF', 'GEMM')
+    WGRAD_KINDS = ('BF', 'STEM', 'HEAD', 'FP32')
+
+    def layer_plan(self, i):
+        """Layer i's planned kernels and views (after bind): {'fwd', 'dgrad', 'wgrad': kernel kind name, 'x', 'y', 'dpre',
+        'dx': torch view [n,h,w,c] into the workspace, dx None when the layer has no input gradient}."""
+        kinds = (c_int * 3)()
+        ptrs = (c_void_p * 4)()
+        dims = (c_int * 20)()
+        check(self._lib.ms_engine_layer_plan(self._h, i, kinds, ptrs, dims), 'layer_plan')
+        out = {'fwd': self.FWD_KINDS[kinds[0]], 'dgrad': self.DGRAD_KINDS[kinds[1]], 'wgrad': self.WGRAD_KINDS[kinds[2]]}
+        for k, role in enumerate(('x', 'y', 'dpre', 'dx')):
+            out[role] = self._view(ptrs[k], *dims[5 * k:5 * k + 5]) if ptrs[k] else None
+        return out
+
     def tensor(self, name):
         """torch view [n,h,w,c] (strided) of an engine tensor inside the workspace."""
         p, (n, h, w, c, cs) = self.tensor_info(name)
+        return self._view(p, n, h, w, c, cs)
+
+    def _view(self, p, n, h, w, c, cs):
         base = self.workspace
         if self._rs_scratch is not None and 0 <= p - self._rs_scratch.data_ptr() < 4 * self._rs_scratch.numel():
             base = self._rs_scratch                   # rs_left / rs_right / rs_proxy / rs_disp
