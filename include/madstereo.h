@@ -92,26 +92,8 @@ int ms_conv2d_wgrad_bf(const float* x, int n, int h, int w, int cin, int x_cs, c
                        int dy_cs, float* dw /*HWIO*/, float* db, int kh, int kw, int stride, int dilation,
                        void* scratch, size_t scratch_bytes, void* stream);
 size_t ms_conv2d_wgrad_bf_scratch(int n, int h, int w, int oh, int ow, int kh, int kw, int cin, int cout);
-/* Plane-level entry points of the same path (what the engine issues per layer in steady state: activations are split
- * by the producing kernel's epilogue, weights once per update).  hi / lo planes: 16-bit NHWC, channel stride `*_pcs`
- * (multiple of 8), fmt 0 = bf16, 1 = fp16 of value * scale (scale a power of two); weight tiles: ms_bf_weight_halfs() 16-bit elements (both planes,
- * pre-tiled shared-memory images); job_dev: >= 64 bytes of device scratch; part / tickets:
- * ms_conv2d_bf_part_floats() floats / ms_conv2d_bf_ticket_words() zeroed words (split-K). */
-int ms_bf_split(const float* x, int n, int h, int w, int c, int x_cs, void* hi, void* lo, int plane_cs, int fmt, float scale,
-                void* stream);
+/* 16-bit elements (both planes) of the pre-tiled weights of an M x K GEMM over `taps` taps on the same path */
 size_t ms_bf_weight_halfs(int taps, int m, int k);
-int ms_bf_prep_weights(const float* weights_hwio, int taps, int cin, int cout, int for_dgrad, int fmt, void* tiles,
-                       void* job_dev, void* stream);
-int ms_conv2d_fwd_bf_planes(const void* xhi, const void* xlo, int x_pcs, int fmt, float scale, int n, int h, int w, int cin,
-                            const void* wtiles, const float* bias, float* y, int cout, int y_cs, void* yhi, void* ylo,
-                            int y_pcs, int kh, int kw, int stride, int dilation, float alpha, float* part,
-                            unsigned int* tickets, void* stream);
-size_t ms_conv2d_bf_part_floats(void);
-size_t ms_conv2d_bf_ticket_words(void);
-int ms_conv2d_wgrad_bf_planes(const void* xhi, const void* xlo, int x_pcs, int n, int h, int w, int cin,
-                              const void* dhi, const void* dlo, int d_pcs, int oh, int ow, int cout, float* dw, float* db,
-                              int kh, int kw, int stride, int dilation, float* workspace, size_t workspace_floats, void* stream);
-size_t ms_conv2d_wgrad_bf_workspace(int kh, int kw, int cin, int cout);
 size_t ms_conv2d_wgrad_workspace(int kh, int kw, int cin, int cout, size_t out_pixels);
 int ms_conv2d_wgrad(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int oh, int ow,
                     int cout, int dy_cs, float* dw /*HWIO*/, float* db, int kh, int kw, int stride,
@@ -205,6 +187,8 @@ int ms_engine_layer_info(void* e, int i, char* name, int name_cap, char* scope, 
 /* Replaces the per-module var_list construction from block_config JSON (Stereo_Online_Adaptation.py:110-118,
  * Nets/Stereo_net.py:213-222): group_of_layer[i] = MAD module index of layer i, or -1. Fixes the arena order. */
 int ms_engine_set_groups(void* e, const int* group_of_layer, int n_layers, int n_groups);
+/* Lays the engine out (no device needed) and checks every layer against the tensors it runs on; ms_engine_bind does the
+ * same.  -2 (ms_last_error names the layer): a layer's tensors do not fit it. */
 int ms_engine_sizes(void* e, size_t* n_param_floats, size_t* workspace_floats);
 int ms_engine_param_offsets(void* e, int i, size_t* w_off, size_t* b_off);
 int ms_engine_group_range(void* e, int g, size_t* begin, size_t* end);

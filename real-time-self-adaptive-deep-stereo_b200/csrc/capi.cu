@@ -10,13 +10,18 @@ namespace ms { const char* last_error_cstr(); }
 using namespace ms;
 
 static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s); }
-static void same_pad_c(int in, int k, int s, int d, int& out, int& before) {
-    int keff = (k - 1) * d + 1;
-    out = (in + s - 1) / s;
-    int total = (out - 1) * s + keff - in;
-    if (total < 0) total = 0;
-    before = total / 2;
+// the layer an entry point's arguments describe, for the geometry functions of engine.h
+static ConvLayer layer(int kh, int kw, int cin, int cout, int stride, int dil, float alpha, int transposed) {
+    ConvLayer L{};
+    L.kh = kh; L.kw = kw; L.cin = cin; L.cout = cout; L.stride = stride; L.dil = dil; L.alpha = alpha; L.transposed = transposed;
+    return L;
 }
+// an [n,h,w,c] view of caller memory, and one of the layer's output size on an h x w input
+static TView in_view(const float* p, int n, int h, int w, int c, int cs) { return view(const_cast<float*>(p), n, h, w, c, cs); }
+static TView out_view(const ConvLayer& L, const float* p, int n, int h, int w, int c, int cs) {
+    return in_view(p, n, conv_out_size(L, h), conv_out_size(L, w), c, cs);
+}
+static int mismatch(const char* fn) { set_error(std::string(fn) + ": shape mismatch"); return -2; }
 static void copy_str(char* dst, int cap, const std::string& s) {
     if (!dst || cap <= 0) return;
     size_t n = std::min((size_t)cap - 1, s.size());
@@ -66,63 +71,41 @@ int ms_corr_bwd(const float* left, int left_cs, const float* right, int right_cs
 
 int ms_conv2d_fwd(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights, const float* bias,
                   float* y, int cout, int y_cs, int kh, int kw, int stride, int dilation, float alpha, void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh, pt);
-    same_pad_c(w, kw, stride, dilation, ow, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    p.y = view(y, n, oh, ow, cout, y_cs);
-    p.wmat = weights; p.bias = bias; p.kh = kh; p.kw = kw;
-    p.mul = stride; p.off_y = -pt; p.off_x = -pl; p.step = dilation; p.div = 1;
-    p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, dilation, alpha, 0);
+    ConvGemm p;
+    if (!conv_fwd_geom(L, in_view(x, n, h, w, cin, x_cs), out_view(L, y, n, h, w, cout, y_cs), p)) return mismatch("ms_conv2d_fwd");
+    p.wmat = weights; p.bias = bias;
     return conv_gemm(p, S(stream));
 }
 
 int ms_conv2d_dgrad(const float* dy, int n, int oh, int ow, int cout, int dy_cs, const float* weights, float* dx,
                     int h, int w, int cin, int dx_cs, int kh, int kw, int stride, int dilation, float* scratch,
                     void* stream) {
-    int oh2, ow2, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh2, pt);
-    same_pad_c(w, kw, stride, dilation, ow2, pl);
-    if (oh2 != oh || ow2 != ow) { set_error("ms_conv2d_dgrad: shape mismatch"); return -2; }
+    ConvGemm p;
+    if (!conv_dgrad_geom(layer(kh, kw, cin, cout, stride, dilation, 1.f, 0), in_view(dy, n, oh, ow, cout, dy_cs),
+                         in_view(dx, n, h, w, cin, dx_cs), p)) return mismatch("ms_conv2d_dgrad");
     if (transpose_taps(weights, scratch, kh * kw, cin, cout, S(stream))) return -1;
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);
-    p.y = view(dx, n, h, w, cin, dx_cs);
-    p.wmat = scratch; p.bias = nullptr; p.kh = kh; p.kw = kw;
-    p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -dilation; p.div = stride;
-    p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    p.wmat = scratch;
     return conv_gemm(p, S(stream));
 }
 
 int ms_conv2d_fwd_bf(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights, const float* bias,
                      float* y, int cout, int y_cs, int kh, int kw, int stride, int dilation, float alpha, float act_scale,
                      void* scratch, size_t scratch_bytes, void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh, pt);
-    same_pad_c(w, kw, stride, dilation, ow, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    p.y = view(y, n, oh, ow, cout, y_cs);
-    p.wmat = weights; p.bias = bias; p.kh = kh; p.kw = kw;
-    p.mul = stride; p.off_y = -pt; p.off_x = -pl; p.step = dilation; p.div = 1;
-    p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, dilation, alpha, 0);
+    ConvGemm p;
+    if (!conv_fwd_geom(L, in_view(x, n, h, w, cin, x_cs), out_view(L, y, n, h, w, cout, y_cs), p)) return mismatch("ms_conv2d_fwd_bf");
+    p.wmat = weights; p.bias = bias;
     if (!conv_bf_supported(p)) { set_error("ms_conv2d_fwd_bf: shape not supported by the split-16-bit tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 0, 1, act_scale, scratch, scratch_bytes, S(stream));      // forward: fp16 planes of x * act_scale
 }
 int ms_conv2d_dgrad_bf(const float* dy, int n, int oh, int ow, int cout, int dy_cs, const float* weights, float* dx,
                        int h, int w, int cin, int dx_cs, int kh, int kw, int stride, int dilation, void* scratch,
                        size_t scratch_bytes, void* stream) {
-    int oh2, ow2, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh2, pt);
-    same_pad_c(w, kw, stride, dilation, ow2, pl);
-    if (oh2 != oh || ow2 != ow) { set_error("ms_conv2d_dgrad_bf: shape mismatch"); return -2; }
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);
-    p.y = view(dx, n, h, w, cin, dx_cs);
-    p.wmat = weights; p.bias = nullptr; p.kh = kh; p.kw = kw;
-    p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -dilation; p.div = stride;
-    p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    ConvGemm p;
+    if (!conv_dgrad_geom(layer(kh, kw, cin, cout, stride, dilation, 1.f, 0), in_view(dy, n, oh, ow, cout, dy_cs),
+                         in_view(dx, n, h, w, cin, dx_cs), p)) return mismatch("ms_conv2d_dgrad_bf");
+    p.wmat = weights;
     if (!conv_bf_supported(p)) { set_error("ms_conv2d_dgrad_bf: shape not supported by the split-16-bit tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 1, 0, 1.f, scratch, scratch_bytes, S(stream));      // gradients: bf16 planes
 }
@@ -136,15 +119,10 @@ size_t ms_conv2d_bf_scratch(int n, int h, int w, int kh, int kw, int cin, int co
 int ms_conv2d_wgrad_bf(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int oh, int ow, int cout,
                        int dy_cs, float* dw, float* db, int kh, int kw, int stride, int dilation, void* scratch,
                        size_t scratch_bytes, void* stream) {
-    int oh2, ow2, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh2, pt);
-    same_pad_c(w, kw, stride, dilation, ow2, pl);
-    if (oh2 != oh || ow2 != ow) { set_error("ms_conv2d_wgrad_bf: shape mismatch"); return -2; }
-    ConvWgrad q{};
-    q.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    q.dy = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);
-    q.dw = dw; q.db = db; q.kh = kh; q.kw = kw; q.stride = stride; q.dil = dilation; q.pad_t = pt; q.pad_l = pl;
-    q.accumulate = 0;
+    ConvWgrad q;
+    if (!conv_wgrad_geom(layer(kh, kw, cin, cout, stride, dilation, 1.f, 0), in_view(x, n, h, w, cin, x_cs),
+                         in_view(dy, n, oh, ow, cout, dy_cs), q)) return mismatch("ms_conv2d_wgrad_bf");
+    q.dw = dw; q.db = db;
     if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_wgrad_bf: shape not supported by the split-16-bit tensor-core path"); return -3; }
     return wgrad_bf_oneshot(q, scratch, scratch_bytes, S(stream));
 }
@@ -153,19 +131,15 @@ size_t ms_conv2d_wgrad_bf_scratch(int n, int h, int w, int oh, int ow, int kh, i
     q.x = view(nullptr, n, h, w, cin, cin); q.dy = view(nullptr, n, oh, ow, cout, cout); q.kh = kh; q.kw = kw;
     return wgrad_bf_oneshot_scratch_bytes(q);
 }
+size_t ms_bf_weight_halfs(int taps, int m, int k) { return conv_bf_weight_halfs(taps, m, k); }
 // ---- DispNet conv1 (7x7 stride 2, 3 -> 64; Nets/DispNet.py:82-86) on the direct CUDA-core kernels (csrc/conv_stem.cu).
 //      x: [n,h,w,3] stored with a channel stride of 4 floats (the engine's padded image layout)
 int ms_conv2d_stem_fwd(const float* x4, int n, int h, int w, const float* weights, const float* bias, float* y, int y_cs,
                        float alpha, void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, 7, 2, 1, oh, pt);
-    same_pad_c(w, 7, 2, 1, ow, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(x4), n, h, w, 3, 4);
-    p.y = view(y, n, oh, ow, 64, y_cs);
-    p.wmat = weights; p.bias = bias; p.kh = 7; p.kw = 7;
-    p.mul = 2; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1;
-    p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    const ConvLayer L = layer(7, 7, 3, 64, 2, 1, alpha, 0);
+    ConvGemm p;
+    if (!conv_fwd_geom(L, in_view(x4, n, h, w, 3, 4), out_view(L, y, n, h, w, 64, y_cs), p)) return mismatch("ms_conv2d_stem_fwd");
+    p.wmat = weights; p.bias = bias;
     if (!conv_stem_fwd_supported(p)) { set_error("ms_conv2d_stem_fwd: unsupported layout"); return -3; }
     return conv_stem_fwd(p, nullptr, S(stream));
 }
@@ -176,51 +150,34 @@ size_t ms_conv2d_stem_wgrad_workspace(int n, int h, int w) {
 }
 int ms_conv2d_stem_wgrad(const float* x4, int n, int h, int w, const float* dy, int dy_cs, float* dw, float* db, float* workspace,
                          size_t workspace_floats, void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, 7, 2, 1, oh, pt);
-    same_pad_c(w, 7, 2, 1, ow, pl);
-    ConvWgrad q{};
-    q.x = view(const_cast<float*>(x4), n, h, w, 3, 4);
-    q.dy = view(const_cast<float*>(dy), n, oh, ow, 64, dy_cs);
-    q.dw = dw; q.db = db; q.kh = q.kw = 7; q.stride = 2; q.dil = 1; q.pad_t = pt; q.pad_l = pl;
-    q.workspace = workspace; q.workspace_floats = workspace_floats; q.accumulate = 0;
+    const ConvLayer L = layer(7, 7, 3, 64, 2, 1, 1.f, 0);
+    ConvWgrad q;
+    if (!conv_wgrad_geom(L, in_view(x4, n, h, w, 3, 4), out_view(L, dy, n, h, w, 64, dy_cs), q)) return mismatch("ms_conv2d_stem_wgrad");
+    q.dw = dw; q.db = db; q.workspace = workspace; q.workspace_floats = workspace_floats;
     if (!conv_stem_wgrad_supported(q)) { set_error("ms_conv2d_stem_wgrad: unsupported layout"); return -3; }
     return conv_stem_wgrad(q, S(stream));
 }
 
 // ---- conv2d_transpose (Nets/sharedLayers.py:80-92) and its two gradients on the split-16-bit tensor-core path.
 //      weights [kh,kw,cout,cin] (TF layout); x [n,h,w,cin]; y / dy [n,h*stride,w*stride,cout]
-static void transpose_geom(int h, int w, int kh, int kw, int stride, int& oh, int& ow, int& pt, int& pl) {
-    oh = h * stride; ow = w * stride;
-    int t0, t1;
-    same_pad_c(oh, kh, stride, 1, t0, pt);
-    same_pad_c(ow, kw, stride, 1, t1, pl);
-}
 int ms_conv2d_transpose_fwd_bf(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights, const float* bias,
                                float* y, int cout, int y_cs, int kh, int kw, int stride, float alpha, float act_scale,
                                void* scratch, size_t scratch_bytes, void* stream) {
-    int oh, ow, pt, pl;
-    transpose_geom(h, w, kh, kw, stride, oh, ow, pt, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    p.y = view(y, n, oh, ow, cout, y_cs);
-    p.wmat = weights; p.bias = bias; p.kh = kh; p.kw = kw;
-    p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = stride;
-    p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, 1, alpha, 1);
+    ConvGemm p;
+    if (!conv_fwd_geom(L, in_view(x, n, h, w, cin, x_cs), out_view(L, y, n, h, w, cout, y_cs), p)) return mismatch("ms_conv2d_transpose_fwd_bf");
+    p.wmat = weights; p.bias = bias;
     if (!conv_bf_supported(p)) { set_error("ms_conv2d_transpose_fwd_bf: shape not supported by the tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 1, 1, act_scale, scratch, scratch_bytes, S(stream));     // [tap][M = cout][K = cin], fp16 planes
 }
 int ms_conv2d_transpose_dgrad_bf(const float* dy, int n, int h, int w, int cout, int dy_cs, const float* weights, float* dx,
                                  int cin, int dx_cs, int kh, int kw, int stride, void* scratch, size_t scratch_bytes,
                                  void* stream) {
-    int oh, ow, pt, pl;
-    transpose_geom(h, w, kh, kw, stride, oh, ow, pt, pl);
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);
-    p.y = view(dx, n, h, w, cin, dx_cs);
-    p.wmat = weights; p.bias = nullptr; p.kh = kh; p.kw = kw;
-    p.mul = stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1;      // = the strided conv of dy with HWIO [.,.,cout,cin]
-    p.alpha = 1.f; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, 1, 1.f, 1);
+    ConvGemm p;
+    if (!conv_dgrad_geom(L, out_view(L, dy, n, h, w, cout, dy_cs), in_view(dx, n, h, w, cin, dx_cs), p))
+        return mismatch("ms_conv2d_transpose_dgrad_bf");
+    p.wmat = weights;                                                  // = the strided conv of dy with HWIO [.,.,cout,cin]
     if (!conv_bf_supported(p)) { set_error("ms_conv2d_transpose_dgrad_bf: shape not supported by the tensor-core path"); return -3; }
     return conv_bf_oneshot(p, 0, 0, 1.f, scratch, scratch_bytes, S(stream));           // [tap][K = cout][M = cin], bf16 planes
 }
@@ -231,85 +188,26 @@ size_t ms_conv2d_transpose_bf_scratch(int n, int h, int w, int kh, int kw, int c
     size_t sa = conv_bf_oneshot_scratch_bytes(a), sb = conv_bf_oneshot_scratch_bytes(b);
     return sa > sb ? sa : sb;
 }
-static ConvWgrad transpose_wgrad_geom(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int cout, int dy_cs,
-                                      int kh, int kw, int stride) {
-    int oh, ow, pt, pl;
-    transpose_geom(h, w, kh, kw, stride, oh, ow, pt, pl);
-    ConvWgrad q{};
-    q.x = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);      // the strided conv's input is the big map ...
-    q.dy = view(const_cast<float*>(x), n, h, w, cin, x_cs);          // ... and its "output gradient" the layer's input
-    q.kh = kh; q.kw = kw; q.stride = stride; q.dil = 1; q.pad_t = pt; q.pad_l = pl; q.accumulate = 0;
-    return q;
-}
 size_t ms_conv2d_transpose_wgrad_bf_scratch(int n, int h, int w, int kh, int kw, int cin, int cout, int stride) {
-    ConvWgrad q = transpose_wgrad_geom(nullptr, n, h, w, cin, cin, nullptr, cout, cout, kh, kw, stride);
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, 1, 1.f, 1);
+    ConvWgrad q;
+    conv_wgrad_geom(L, in_view(nullptr, n, h, w, cin, cin), out_view(L, nullptr, n, h, w, cout, cout), q);    // fits: sized from L
     return wgrad_bf_oneshot_scratch_bytes(q);
 }
 int ms_conv2d_transpose_wgrad_bf(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int cout, int dy_cs,
                                  float* dw, float* db, int kh, int kw, int stride, void* scratch, size_t scratch_bytes,
                                  void* stream) {
-    ConvWgrad q = transpose_wgrad_geom(x, n, h, w, cin, x_cs, dy, cout, dy_cs, kh, kw, stride);
-    q.dw = dw; q.db = nullptr;                                        // dw [kh,kw,cout,cin]
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, 1, 1.f, 1);
+    ConvWgrad q;      // the strided conv's input is the big map dy, its "output gradient" the layer's input x
+    if (!conv_wgrad_geom(L, in_view(x, n, h, w, cin, x_cs), out_view(L, dy, n, h, w, cout, dy_cs), q))
+        return mismatch("ms_conv2d_transpose_wgrad_bf");
+    q.dw = dw;                                                        // dw [kh,kw,cout,cin]
     if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_transpose_wgrad_bf: shape not supported by the tensor-core path"); return -3; }
     if (wgrad_bf_oneshot(q, scratch, scratch_bytes, S(stream))) return -1;
     if (!db) return 0;
     // bias gradient = per-channel sum of dy; the partial-sum region of the scratch is free again after the reduction
     return bias_grad(q.x, db, static_cast<float*>(scratch), scratch_bytes / sizeof(float), S(stream));
 }
-// ---- plane-level entry points of the split-bf16 path: what the engine calls per layer in steady state (operands
-//      already split: activations by the producing epilogue, weights once per update)
-int ms_bf_split(const float* x, int n, int h, int w, int c, int x_cs, void* hi, void* lo, int plane_cs, int fmt, float scale,
-                void* stream) {
-    ActPlanes pl; pl.hi = hi; pl.lo = lo; pl.cs = plane_cs; pl.fmt = fmt; pl.scale = fmt == 1 ? scale : 1.f;
-    return split_planes(view(const_cast<float*>(x), n, h, w, c, x_cs), pl, S(stream));
-}
-size_t ms_bf_weight_halfs(int taps, int m, int k) { return conv_bf_weight_halfs(taps, m, k); }
-int ms_bf_prep_weights(const float* weights_hwio, int taps, int cin, int cout, int for_dgrad, int fmt, void* tiles,
-                       void* job_dev, void* stream) {
-    const int M = for_dgrad ? cin : cout, K = for_dgrad ? cout : cin;
-    int Mpad, Kpad; conv_bf_weight_dims(M, K, Mpad, Kpad);
-    BfPrepJob job{weights_hwio, tiles, taps, M, K, Mpad, Kpad, for_dgrad ? 0 : 1, fmt};
-    MS_CHECK_CUDA(cudaMemcpyAsync(job_dev, &job, sizeof job, cudaMemcpyHostToDevice, S(stream)));
-    MS_CHECK_CUDA(cudaStreamSynchronize(S(stream)));
-    return bf_prep_weights(static_cast<const BfPrepJob*>(job_dev), 1, conv_bf_weight_halfs(taps, M, K), S(stream));
-}
-int ms_conv2d_fwd_bf_planes(const void* xhi, const void* xlo, int x_pcs, int fmt, float scale, int n, int h, int w, int cin,
-                            const void* wtiles, const float* bias, float* y, int cout, int y_cs, void* yhi, void* ylo,
-                            int y_pcs, int kh, int kw, int stride, int dilation, float alpha, float* part,
-                            unsigned int* tickets, void* stream) {
-    int oh, ow, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh, pt);
-    same_pad_c(w, kw, stride, dilation, ow, pl);
-    ConvGemm p{};
-    p.x = view(nullptr, n, h, w, cin, cin);
-    p.y = view(y, n, oh, ow, cout, y_cs);
-    p.bias = bias; p.kh = kh; p.kw = kw;
-    p.mul = stride; p.off_y = -pt; p.off_x = -pl; p.step = dilation; p.div = 1;
-    p.alpha = alpha; p.mask_alpha = 1.f;
-    if (!conv_bf_supported(p)) { set_error("ms_conv2d_fwd_bf_planes: shape not supported"); return -3; }
-    ActPlanes xp; xp.hi = const_cast<void*>(xhi); xp.lo = const_cast<void*>(xlo); xp.cs = x_pcs; xp.fmt = fmt; xp.scale = fmt == 1 ? scale : 1.f;
-    ActPlanes yp; yp.hi = yhi; yp.lo = ylo; yp.cs = y_pcs; yp.fmt = fmt; yp.scale = xp.scale;
-    return conv_bf(p, xp, wtiles, yhi ? &yp : nullptr, part, tickets, S(stream));
-}
-size_t ms_conv2d_bf_part_floats() { return conv_bf_part_floats(); }
-size_t ms_conv2d_bf_ticket_words() { return conv_bf_ticket_words(); }
-int ms_conv2d_wgrad_bf_planes(const void* xhi, const void* xlo, int x_pcs, int n, int h, int w, int cin,
-                              const void* dhi, const void* dlo, int d_pcs, int oh, int ow, int cout, float* dw, float* db,
-                              int kh, int kw, int stride, int dilation, float* workspace, size_t workspace_floats, void* stream) {
-    int oh2, ow2, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh2, pt);
-    same_pad_c(w, kw, stride, dilation, ow2, pl);
-    if (oh2 != oh || ow2 != ow) { set_error("ms_conv2d_wgrad_bf_planes: shape mismatch"); return -2; }
-    ConvWgrad q{};
-    q.x = view(nullptr, n, h, w, cin, cin); q.dy = view(nullptr, n, oh, ow, cout, cout);
-    q.dw = dw; q.db = db; q.kh = kh; q.kw = kw; q.stride = stride; q.dil = dilation; q.pad_t = pt; q.pad_l = pl;
-    q.workspace = workspace; q.workspace_floats = workspace_floats;
-    if (!wgrad_bf_supported(q)) { set_error("ms_conv2d_wgrad_bf_planes: shape not supported"); return -3; }
-    ActPlanes xp; xp.hi = const_cast<void*>(xhi); xp.lo = const_cast<void*>(xlo); xp.cs = x_pcs; xp.fmt = 0; xp.scale = 1.f;
-    ActPlanes dp; dp.hi = const_cast<void*>(dhi); dp.lo = const_cast<void*>(dlo); dp.cs = d_pcs; dp.fmt = 0; dp.scale = 1.f;
-    return wgrad_bf(q, xp, dp, S(stream));
-}
-size_t ms_conv2d_wgrad_bf_workspace(int kh, int kw, int cin, int cout) { return wgrad_bf_workspace_floats(kh, kw, cin, cout); }
 
 size_t ms_conv2d_wgrad_workspace(int kh, int kw, int cin, int cout, size_t out_pixels) {
     return conv_wgrad_workspace_floats(kh * kw, cin, cout, out_pixels);
@@ -318,32 +216,21 @@ size_t ms_conv2d_wgrad_workspace(int kh, int kw, int cin, int cout, size_t out_p
 int ms_conv2d_wgrad(const float* x, int n, int h, int w, int cin, int x_cs, const float* dy, int oh, int ow, int cout,
                     int dy_cs, float* dw, float* db, int kh, int kw, int stride, int dilation, float* workspace,
                     size_t workspace_floats, void* stream) {
-    int oh2, ow2, pt, pl;
-    same_pad_c(h, kh, stride, dilation, oh2, pt);
-    same_pad_c(w, kw, stride, dilation, ow2, pl);
-    if (oh2 != oh || ow2 != ow) { set_error("ms_conv2d_wgrad: shape mismatch"); return -2; }
-    ConvWgrad q{};
-    q.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    q.dy = view(const_cast<float*>(dy), n, oh, ow, cout, dy_cs);
-    q.dw = dw; q.db = db; q.kh = kh; q.kw = kw; q.stride = stride; q.dil = dilation; q.pad_t = pt; q.pad_l = pl;
-    q.workspace = workspace; q.workspace_floats = workspace_floats; q.accumulate = 0;
+    ConvWgrad q;
+    if (!conv_wgrad_geom(layer(kh, kw, cin, cout, stride, dilation, 1.f, 0), in_view(x, n, h, w, cin, x_cs),
+                         in_view(dy, n, oh, ow, cout, dy_cs), q)) return mismatch("ms_conv2d_wgrad");
+    q.dw = dw; q.db = db; q.workspace = workspace; q.workspace_floats = workspace_floats;
     return conv_wgrad(q, S(stream));
 }
 
 int ms_conv2d_transpose_fwd(const float* x, int n, int h, int w, int cin, int x_cs, const float* weights,
                             const float* bias, float* y, int cout, int y_cs, int kh, int kw, int stride, float alpha,
                             float* scratch, void* stream) {
-    const int oh = h * stride, ow = w * stride;
-    int t0, t1, pt, pl;
-    same_pad_c(oh, kh, stride, 1, t0, pt);
-    same_pad_c(ow, kw, stride, 1, t1, pl);
+    const ConvLayer L = layer(kh, kw, cin, cout, stride, 1, alpha, 1);
+    ConvGemm p;
+    if (!conv_fwd_geom(L, in_view(x, n, h, w, cin, x_cs), out_view(L, y, n, h, w, cout, y_cs), p)) return mismatch("ms_conv2d_transpose_fwd");
     if (transpose_taps(weights, scratch, kh * kw, cout, cin, S(stream))) return -1;   // [tap][cout][cin] -> [tap][cin][cout]
-    ConvGemm p{};
-    p.x = view(const_cast<float*>(x), n, h, w, cin, x_cs);
-    p.y = view(y, n, oh, ow, cout, y_cs);
-    p.wmat = scratch; p.bias = bias; p.kh = kh; p.kw = kw;
-    p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = stride;
-    p.alpha = alpha; p.mask = nullptr; p.mask_alpha = 1.f; p.res = nullptr; p.accumulate = 0;
+    p.wmat = scratch; p.bias = bias;
     return conv_gemm(p, S(stream));
 }
 
@@ -428,8 +315,7 @@ int ms_engine_set_groups(void* h, const int* group_of_layer, int n_layers, int n
 int ms_engine_sizes(void* h, size_t* n_param_floats, size_t* workspace_floats) {
     Engine* e = static_cast<Engine*>(h);
     if (n_param_floats) *n_param_floats = e->n_params;
-    if (workspace_floats) *workspace_floats = e->layout(nullptr);
-    return 0;
+    return workspace_floats ? e->layout(nullptr, workspace_floats) : 0;
 }
 int ms_engine_param_offsets(void* h, int i, size_t* w_off, size_t* b_off) {
     Engine* e = static_cast<Engine*>(h);
@@ -446,13 +332,15 @@ int ms_engine_group_range(void* h, int g, size_t* begin, size_t* end) {
 int ms_engine_bind(void* h, float* weights, float* grads, float* momentum, float* workspace, size_t workspace_floats,
                    void* stream) {
     Engine* e = static_cast<Engine*>(h);
-    size_t need = e->layout(nullptr);
+    size_t need, used;
+    if (e->layout(nullptr, &need)) return -2;
     if (workspace_floats < need) { set_error("ms_engine_bind: workspace too small"); return -2; }
     if (((uintptr_t)weights | (uintptr_t)grads | (uintptr_t)momentum | (uintptr_t)workspace) & 255) {
         set_error("ms_engine_bind: arenas must be 256-byte aligned"); return -2;
     }
     e->Wt = weights; e->Gr = grads; e->Mo = momentum; e->ws = workspace; e->ws_floats = workspace_floats;
-    if (e->layout(workspace) > need) { set_error("ms_engine_bind: layout exceeds the size reported by ms_engine_sizes"); return -2; }
+    if (e->layout(workspace, &used)) return -2;
+    if (used > need) { set_error("ms_engine_bind: layout exceeds the size reported by ms_engine_sizes"); return -2; }
     MS_CHECK_CUDA(cudaMemsetAsync(workspace, 0, need * sizeof(float), S(stream)));
     MS_CHECK_CUDA(cudaMemsetAsync(grads, 0, e->n_params * sizeof(float), S(stream)));
     if (!e->bf_jobs.empty())

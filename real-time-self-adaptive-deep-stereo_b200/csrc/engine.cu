@@ -93,40 +93,58 @@ static bool conv_pads(const ConvLayer& L, const TView& in, const TView& out, int
     return oh == out.h && ow == out.w;
 }
 
-// Kernel arguments of a layer's three directions, shared by the planner and the dispatch so that both put the same
-// question to the kernels' predicates.  false: the views do not fit the layer.
-bool Engine::fwd_args(const ConvLayer& L, const TView& x, const TView& y, ConvGemm& p) const {
+bool conv_fwd_geom(const ConvLayer& L, const TView& x, const TView& y, ConvGemm& p) {
     p = ConvGemm{};
     p.x = x; p.y = y; p.kh = L.kh; p.kw = L.kw;
-    p.bias = Wt + L.b_off; p.alpha = L.alpha; p.mask_alpha = 1.f;
-    p.part = sk().gemm_part; p.part_floats = conv_gemm_part_floats();
+    p.alpha = L.alpha; p.mask_alpha = 1.f;
     int pt, pl;
     const bool ok = L.transposed ? conv_pads(L, y, x, pt, pl) : conv_pads(L, x, y, pt, pl);
-    if (!L.transposed) { p.wmat = Wt + L.w_off; p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = L.dil; p.div = 1; }
-    // canonical W of a transposed layer is [tap][cout][cin]; the gather GEMM wants [tap][K=cin][N=cout] (transpose_taps)
-    else { p.wmat = wT; p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = L.stride; }
+    if (!L.transposed) { p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = L.dil; p.div = 1; }
+    else { p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -1; p.div = L.stride; }
     return ok && x.c == L.cin && y.c == L.cout;
 }
 // input gradient: the gather of dpre (a transposed layer: the stride-s conv of dpre with its canonical weights)
-bool Engine::dgrad_args(const ConvLayer& L, const TView& dpre, const TView& dx, ConvGemm& p) const {
+bool conv_dgrad_geom(const ConvLayer& L, const TView& dpre, const TView& dx, ConvGemm& p) {
     p = ConvGemm{};
-    p.x = dpre; p.y = dx; p.wmat = Wt + L.w_off; p.kh = L.kh; p.kw = L.kw;
+    p.x = dpre; p.y = dx; p.kh = L.kh; p.kw = L.kw;
     p.alpha = 1.f; p.mask_alpha = 1.f;
-    p.part = sk().gemm_part; p.part_floats = conv_gemm_part_floats();
     int pt, pl;
     const bool ok = L.transposed ? conv_pads(L, dpre, dx, pt, pl) : conv_pads(L, dx, dpre, pt, pl);
     if (L.transposed) { p.mul = L.stride; p.off_y = -pt; p.off_x = -pl; p.step = 1; p.div = 1; }
     else { p.mul = 1; p.off_y = pt; p.off_x = pl; p.step = -L.dil; p.div = L.stride; }
     return ok && dpre.c == L.cout && dx.c == L.cin;
 }
-// weight gradient (a transposed layer: of the stride-s conv from its output-sized dpre to its input x; bias separately)
-bool Engine::wgrad_args(const ConvLayer& L, const TView& x, const TView& dpre, ConvWgrad& q) const {
+// weight gradient (a transposed layer: of the stride-s conv from its output-sized dpre to its input x)
+bool conv_wgrad_geom(const ConvLayer& L, const TView& x, const TView& dpre, ConvWgrad& q) {
     q = ConvWgrad{};
     q.x = L.transposed ? dpre : x; q.dy = L.transposed ? x : dpre;
-    q.dw = Gr + L.w_off; q.db = L.transposed ? nullptr : Gr + L.b_off;
     q.kh = L.kh; q.kw = L.kw; q.stride = L.stride; q.dil = L.dil;
-    q.workspace = wg_ws; q.workspace_floats = wg_ws_floats;
     return conv_pads(L, q.x, q.dy, q.pad_t, q.pad_l) && x.c == L.cin && dpre.c == L.cout;
+}
+
+// The engine's pointers on top of that geometry, shared by the planner and the dispatch so that both put the same
+// question to the kernels' predicates.
+bool Engine::fwd_args(int li, ConvGemm& p) const {
+    const ConvLayer& L = layers[li];
+    const bool ok = conv_fwd_geom(L, plan[li].x, plan[li].y, p);
+    // canonical W of a transposed layer is [tap][cout][cin]; the gather GEMM wants [tap][K=cin][N=cout] (transpose_taps)
+    p.wmat = L.transposed ? wT : Wt + L.w_off; p.bias = Wt + L.b_off;
+    p.part = sk().gemm_part; p.part_floats = conv_gemm_part_floats();
+    return ok;
+}
+bool Engine::dgrad_args(int li, ConvGemm& p) const {
+    const ConvLayer& L = layers[li];
+    const bool ok = conv_dgrad_geom(L, plan[li].dpre, plan[li].dx, p);
+    p.wmat = Wt + L.w_off;
+    p.part = sk().gemm_part; p.part_floats = conv_gemm_part_floats();
+    return ok;
+}
+bool Engine::wgrad_args(int li, ConvWgrad& q) const {
+    const ConvLayer& L = layers[li];
+    const bool ok = conv_wgrad_geom(L, plan[li].x, plan[li].dpre, q);
+    q.dw = Gr + L.w_off; q.db = L.transposed ? nullptr : Gr + L.b_off;      // a transposed layer's bias: bias_grad
+    q.workspace = wg_ws; q.workspace_floats = wg_ws_floats;
+    return ok;
 }
 
 void Engine::prof_reset() {
@@ -256,16 +274,16 @@ void Engine::plan_views(int li, const TView& x, const TView& y, const TView& dpr
 // Every layer's kernels, in order of preference, from the views plan_views() recorded; then what they read: weight
 // tiles and prep jobs of BF forwards and dgrads, fp16 planes of BF forward inputs, bf16 planes of the output gradients
 // of BF dgrads and weight gradients, and the sizes of the weight-gradient workspace, its re-split scratch planes and
-// the transposed-weight scratch.
-void Engine::plan_convs(Bump& A, size_t& max_wg, size_t& max_wt) {
+// the transposed-weight scratch.  -2: a layer's views do not fit it.
+int Engine::plan_convs(Bump& A, size_t& max_wg, size_t& max_wt) {
     wg_xp_halfs = 0;
     for (size_t li = 0; li < layers.size(); ++li) {
         const ConvLayer& L = layers[li];
         ConvPlan& P = plan[li];
         ConvGemm f, d;
         ConvWgrad q;
-        fwd_args(L, P.x, P.y, f);
-        wgrad_args(L, P.x, P.dpre, q);
+        MS_REQUIRE(fwd_args((int)li, f) && wgrad_args((int)li, q) && (!P.dx.p || dgrad_args((int)li, d)),
+                   "layer " + std::to_string(li) + " (" + L.name + "): its planned views do not fit it");
         if (conv_head_kind(f) == 1) P.fwd = ConvPlan::FWD_HEAD;
         else if (conv_one_channel_supported(f)) P.fwd = ConvPlan::FWD_ONE_CHANNEL;
         else if (!L.transposed && conv_stem_fwd_supported(f)) P.fwd = ConvPlan::FWD_STEM;
@@ -278,7 +296,7 @@ void Engine::plan_convs(Bump& A, size_t& max_wg, size_t& max_wt) {
         //  its dgrad and weight gradient stay in fp32)
         const bool dpre_planes = (reinterpret_cast<uintptr_t>(P.dpre.p) & 15) == 0;
         P.dgrad = ConvPlan::DGRAD_GEMM;
-        if (P.dx.p && dgrad_args(L, P.dpre, P.dx, d)) {
+        if (P.dx.p) {
             if (conv_head_kind(d) == 2) P.dgrad = ConvPlan::DGRAD_HEAD;
             else if (dpre_planes && conv_bf_supported(d)) P.dgrad = ConvPlan::DGRAD_BF;
         }
@@ -343,9 +361,11 @@ void Engine::plan_convs(Bump& A, size_t& max_wg, size_t& max_wt) {
         }
         bf_job_end[gidx] = (int)bf_jobs.size();
     }
+    return 0;
 }
 
-size_t Engine::layout(float* base) {
+int Engine::layout(float* base, size_t* floats) {
+    *floats = 0;
     // the sizing pass lays out against a stand-in base with the workspace's 256-byte alignment (never dereferenced), so
     // that both passes plan from the same views
     Bump A{base ? base : reinterpret_cast<float*>(uintptr_t{256}), 0};
@@ -424,7 +444,7 @@ size_t Engine::layout(float* base) {
     g_disp = tens(B, H, W, 1);
     tensors["grad/disp"] = g_disp;
     size_t max_wg = 0, max_wt = 0;
-    plan_convs(A, max_wg, max_wt);
+    if (plan_convs(A, max_wg, max_wt)) return -2;
     wT_floats = max_wt; wT = alloc(max_wt);
     wg_ws_floats = max_wg; wg_ws = alloc(max_wg);
     if (wg_xp_halfs) {
@@ -454,18 +474,19 @@ size_t Engine::layout(float* base) {
         if (module_gemm) splitk[1].gemm_part = alloc(conv_gemm_part_floats());
         loss_full_ws = alloc(loss_value_workspace_floats(B, H, W));
     }
-    return A.off;
+    *floats = A.off;
+    return 0;
 }
 
 // ---------------------------------------------------------------------------------------------
 // conv helpers
 // ---------------------------------------------------------------------------------------------
-int Engine::conv_fwd(const ConvLayer& L, const TView& x, const TView& y, const float* res, int res_cs,
-                     cudaStream_t st) {
-    const int li = (int)(&L - &layers[0]);
+// (every *_args call below fits: plan_convs checked each layer's views at layout time)
+int Engine::conv_fwd(int li, const float* res, int res_cs, cudaStream_t st) {
+    const ConvLayer& L = layers[li];
     const ConvPlan& P = plan[li];
     ConvGemm p;
-    MS_REQUIRE(same_view(x, P.x) && same_view(y, P.y) && fwd_args(L, x, y, p), "conv_fwd: views differ from the layer's plan");
+    fwd_args(li, p);
     p.res = res; p.res_cs = res_cs;
     if (L.transposed && P.fwd != ConvPlan::FWD_BF && transpose_taps(Wt + L.w_off, wT, L.kh * L.kw, L.cout, L.cin, st)) return -1;
     prof_begin(CAT_CONV_FWD, st, li);
@@ -479,14 +500,14 @@ int Engine::conv_fwd(const ConvLayer& L, const TView& x, const TView& y, const f
     case ConvPlan::FWD_STEM: rc = conv_stem_fwd(p, P.yp, st); break;
     case ConvPlan::FWD_SMALL: rc = conv_small_fwd(p, st); break;
     case ConvPlan::FWD_BF:
-        rc = ensure_planes(x, P.xp, st);
+        rc = ensure_planes(P.x, P.xp, st);
         if (!rc) rc = conv_bf(p, *P.xp, P.tiles[0], P.yp, sk().bf_part, sk().bf_tickets, st);
         break;
     default: rc = conv_gemm(p, st);
     }
-    planes_written(y, P.yp, P.fwd == ConvPlan::FWD_STEM || P.fwd == ConvPlan::FWD_BF);
+    planes_written(P.y, P.yp, P.fwd == ConvPlan::FWD_STEM || P.fwd == ConvPlan::FWD_BF);
     prof_end(st);
-    prof_note((double)y.pixels() * L.kh * L.kw * L.cin * L.cout / (L.transposed ? L.stride * L.stride : 1), 0);
+    prof_note((double)P.y.pixels() * L.kh * L.kw * L.cin * L.cout / (L.transposed ? L.stride * L.stride : 1), 0);
     return rc;
 }
 
@@ -507,37 +528,38 @@ int Engine::wgrad(const ConvLayer& L, const ConvPlan& P, const ConvWgrad& q, cud
     }
 }
 
-// x: forward input of the layer; dpre: grad wrt pre-activation output; dx: where to write grad wrt x
-int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, const TView* dx_mask,
-                     float mask_alpha, int dx_acc, int want_wgrad, cudaStream_t st) {
-    const int li = (int)(&L - &layers[0]);
+// from the planned output gradient P.dpre (wrt the pre-activation output): the weight gradient (want_wgrad) and the
+// input gradient into P.dx (want_dx; dx_acc: added to P.dx; dx_slope != 1: masked by the leaky ReLU of P.x, that slope)
+int Engine::conv_bwd(int li, int want_dx, float dx_slope, int dx_acc, int want_wgrad, cudaStream_t st) {
+    const ConvLayer& L = layers[li];
     const ConvPlan& P = plan[li];
     MS_REQUIRE(!L.transposed, "conv_bwd: transposed layers use deconv_bwd");
+    MS_REQUIRE(!want_dx || P.dx.p, "conv_bwd: layer " + L.name + " has no planned input gradient");
     ConvWgrad q;
     ConvGemm p;
-    MS_REQUIRE(same_view(x, P.x) && same_view(dpre, P.dpre) && wgrad_args(L, x, dpre, q) &&
-               (!dx || (same_view(*dx, P.dx) && dgrad_args(L, dpre, *dx, p))), "conv_bwd: views differ from the layer's plan");
+    wgrad_args(li, q);
+    if (want_dx) dgrad_args(li, p);
     if (net == 1) fresh.clear();    // DispNet's backward mutates gradient tensors in place between convs: always re-split
     if (want_wgrad) {
         prof_begin(CAT_CONV_WGRAD, st, li);
         // the planes of dpre also feed the dgrad below: they are produced on `st` BEFORE the fork
-        int rc = P.wgrad == ConvPlan::WGRAD_BF ? ensure_planes(dpre, P.dp, st) : 0;
+        int rc = P.wgrad == ConvPlan::WGRAD_BF ? ensure_planes(P.dpre, P.dp, st) : 0;
         cudaStream_t ws = st;
         if (!rc) rc = fork_wgrad(st, &ws);
         if (!rc) rc = wgrad(L, P, q, ws);
         prof_end(st);
-        prof_note((double)dpre.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
+        prof_note((double)P.dpre.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
     }
-    if (dx) {
-        p.mask = dx_mask ? dx_mask->p : nullptr; p.mask_cs = dx_mask ? dx_mask->cs : 0; p.mask_alpha = mask_alpha;
+    if (want_dx) {
+        if (dx_slope != 1.f) { p.mask = P.x.p; p.mask_cs = P.x.cs; p.mask_alpha = dx_slope; }
         p.accumulate = dx_acc;
         prof_begin(CAT_CONV_DGRAD, st, li);
         int rc;
         switch (P.dgrad) {
         case ConvPlan::DGRAD_HEAD: rc = conv_head(p, st); break;    // [tap][cin][1] == [tap][1][cin]: canonical weights
         case ConvPlan::DGRAD_BF:
-            rc = ensure_planes(dpre, P.dp, st);
+            rc = ensure_planes(P.dpre, P.dp, st);
             if (!rc) rc = conv_bf(p, *P.dp, P.tiles[1], P.dxp, sk().bf_part, sk().bf_tickets, st);
             break;
         default:
@@ -545,9 +567,9 @@ int Engine::conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, cons
             rc = transpose_taps(Wt + L.w_off, wT, L.kh * L.kw, L.cin, L.cout, st);   // -> [tap][cout][cin]
             if (!rc) rc = conv_gemm(p, st);
         }
-        planes_written(*dx, P.dxp, P.dgrad == ConvPlan::DGRAD_BF);
+        planes_written(P.dx, P.dxp, P.dgrad == ConvPlan::DGRAD_BF);
         prof_end(st);
-        prof_note((double)dpre.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
+        prof_note((double)P.dpre.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
     }
     return 0;
@@ -730,11 +752,8 @@ int Engine::forward(int disp_mask, cudaStream_t st, int fork_group, cudaStream_t
         weights_dirty = false;
     }
     if (net == 1) return forward_dispnet(disp_mask, st);
-    TView x = img;
-    for (int i = 1; i <= 12; ++i) {
-        if (conv_fwd(layers[i - 1], x, pyr[i], nullptr, 0, st)) return -1;
-        x = pyr[i];
-    }
+    for (int i = 1; i <= 12; ++i)
+        if (conv_fwd(i - 1, nullptr, 0, st)) return -1;
     for (int k = 6; k >= 2; --k) {
         const int f = feat_of(k), C = PYR_CH[f];
         TView Lf = batch(pyr[f], 0, B), Rf = batch(pyr[f], B, B);
@@ -757,23 +776,13 @@ int Engine::forward(int disp_mask, cudaStream_t st, int fork_group, cudaStream_t
         prof_end(st);
         prof_note(0, (double)B * cf.h * cf.w * (3.0 * C + nd + (cf.u_chan ? 1 : 0) + (cf.out2 ? C : 0)) * 4.0);   // reads L, R(, u); writes corr + the left copy (fused concat)
         if (crc) return -1;
-        TView xin = cost[k];
-        for (int j = 1; j <= 6; ++j) {
-            TView y = (j < 6) ? est[k][j] : V[k];
-            if (conv_fwd(layers[est_layer(k, j)], xin, y, nullptr, 0, st)) return -1;
-            xin = y;
-        }
+        for (int j = 1; j <= 6; ++j)
+            if (conv_fwd(est_layer(k, j), nullptr, 0, st)) return -1;
         if (branch && fork_group == 6 - k && fork()) return -1;
     }
-    {
-        TView xin = ctxin;
-        for (int j = 1; j <= 7; ++j) {
-            TView y = (j < 7) ? ctx[j] : final_;
-            if (conv_fwd(layers[ctx_layer(j)], xin, y, j == 7 ? V[2].p : nullptr, V[2].cs, st)) return -1;
-            xin = y;
-        }
-        if (branch && fork_group == 4 && fork()) return -1;
-    }
+    for (int j = 1; j <= 7; ++j)
+        if (conv_fwd(ctx_layer(j), j == 7 ? V[2].p : nullptr, V[2].cs, st)) return -1;
+    if (branch && fork_group == 4 && fork()) return -1;
     for (int i = 0; i < 6; ++i) {
         if (!(disp_mask & (1 << i))) continue;
         const TView& src = (i < 4) ? V[6 - i] : final_;
@@ -890,33 +899,21 @@ int Engine::backward_impl(int mode, int group, cudaStream_t st) {
 
     // ---- estimator chain of level k: dpre(V_k) in g_V[k] -> (optionally) g_cost[k]
     auto est_bwd = [&](int k, bool need_cost_grad) -> int {
-        TView dpre = g_V[k];
         for (int j = 6; j >= 1; --j) {
             const int li = est_layer(k, j);
-            TView xin = (j == 1) ? cost[k] : est[k][j - 1];
             bool need_dx = (j > 1) ? (need_cost_grad || any_trainable(est_layer(k, 1), li - 1)) : need_cost_grad;
-            TView dx = (j > 1) ? g_est[k][j - 1] : g_cost[k];
-            TView mask = (j > 1) ? est[k][j - 1] : cost[k];
-            if (conv_bwd(layers[li], xin, dpre, need_dx ? &dx : nullptr, (j > 1) ? &mask : nullptr, MAD_ALPHA, 0,
-                         trainable(li, mode, group), st)) return -1;
+            if (conv_bwd(li, need_dx, j > 1 ? MAD_ALPHA : 1.f, 0, trainable(li, mode, group), st)) return -1;
             if (!need_dx) break;
-            dpre = dx;
         }
         return 0;
     };
     // ---- context chain: g_final -> g_ctxin
     auto ctx_bwd = [&](bool need_in_grad) -> int {
-        TView dpre = g_final;
         for (int j = 7; j >= 1; --j) {
             const int li = ctx_layer(j);
-            TView xin = (j == 1) ? ctxin : ctx[j - 1];
             bool need_dx = (j > 1) ? (need_in_grad || any_trainable(ctx_layer(1), li - 1)) : need_in_grad;
-            TView dx = (j > 1) ? g_ctx[j - 1] : g_ctxin;
-            TView mask = (j > 1) ? ctx[j - 1] : ctxin;
-            if (conv_bwd(layers[li], xin, dpre, need_dx ? &dx : nullptr, (j > 1) ? &mask : nullptr, MAD_ALPHA, 0,
-                         trainable(li, mode, group), st)) return -1;
+            if (conv_bwd(li, need_dx, j > 1 ? MAD_ALPHA : 1.f, 0, trainable(li, mode, group), st)) return -1;
             if (!need_dx) break;
-            dpre = dx;
         }
         return 0;
     };
@@ -947,14 +944,10 @@ int Engine::backward_impl(int mode, int group, cudaStream_t st) {
         if (leaky_bwd(g_pyr[top].p, g_pyr[top].cs, pyr[top].p, pyr[top].cs, g_pyr[top].pixels(), g_pyr[top].c,
                       MAD_ALPHA, st)) return -1;
         for (int i = top; i >= lo; --i) {
-            TView xin = (i > 1) ? pyr[i - 1] : img;
             bool need_dx = i > lo;
             int acc = 0;
             if (need_dx && accumulate_feats && (i - 1) >= 4 && ((i - 1) % 2 == 0)) acc = 1;
-            TView dx = g_pyr[i > 1 ? i - 1 : 1];
-            TView mask = pyr[i > 1 ? i - 1 : 1];
-            if (conv_bwd(layers[i - 1], xin, g_pyr[i], need_dx ? &dx : nullptr, need_dx ? &mask : nullptr, MAD_ALPHA,
-                         acc, trainable(i - 1, mode, group), st)) return -1;
+            if (conv_bwd(i - 1, need_dx, MAD_ALPHA, acc, trainable(i - 1, mode, group), st)) return -1;
         }
         return 0;
     };

@@ -23,6 +23,16 @@ struct ConvLayer {
     int group;            // MAD module index or -1
 };
 
+// The gather-GEMM encoding of a layer's three directions on the given views: SAME padding, the mul / off / step / div of
+// the gather (a transposed layer's forward: the fractionally strided case) and the swapped operands of a transposed
+// layer's weight gradient.  Fills the geometry fields and alpha and no pointer but the views'; false: the views do not
+// fit the layer.  The engine and the per-op entry points (capi.cu) build every convolution from these.
+bool conv_fwd_geom(const ConvLayer& L, const TView& x, const TView& y, ConvGemm& p);
+bool conv_dgrad_geom(const ConvLayer& L, const TView& dpre, const TView& dx, ConvGemm& p);
+bool conv_wgrad_geom(const ConvLayer& L, const TView& x, const TView& dpre, ConvWgrad& q);
+// rows (columns) of the layer's output on `in` input rows (columns)
+inline int conv_out_size(const ConvLayer& L, int in) { return L.transposed ? in * L.stride : (in + L.stride - 1) / L.stride; }
+
 constexpr int DP_MAX_WORLD = 8;
 struct DpState {               // device-resident exchange state of one rank (IPC-mapped into every peer), csrc/dp.cu
     unsigned int ready[DP_MAX_WORLD];   // ready[src] = (epoch << 8) | module tag, written by rank src
@@ -47,10 +57,6 @@ struct Bump {            // workspace bump allocator
     float* alloc(size_t n) { float* p = base + off; off += (n + 63) / 64 * 64; return p; }
     TView tens(int n, int h, int w, int c, int cs = 0) { cs = cs ? cs : c; return view(alloc((size_t)n * h * w * cs), n, h, w, c, cs); }
 };
-
-inline bool same_view(const TView& a, const TView& b) {
-    return a.p == b.p && a.n == b.n && a.h == b.h && a.w == b.w && a.c == b.c && a.cs == b.cs;
-}
 
 // byte offset of the right frame in the uint8 staging buffer: the left frame's n bytes rounded up to 4
 inline size_t u8_stage_right_offset(size_t n) { return (n + 3) & ~(size_t)3; }
@@ -120,7 +126,7 @@ struct Engine {
     // ---- per-layer kernel plan (ConvPlan) and the split-16-bit wgmma path (conv_bf.cu, wgrad_bf.cu)
     std::vector<ConvPlan> plan;                    // per layer, filled by layout()
     void plan_views(int li, const TView& x, const TView& y, const TView& dpre, const TView& dx);
-    void plan_convs(Bump& A, size_t& max_wg, size_t& max_wt);
+    int plan_convs(Bump& A, size_t& max_wg, size_t& max_wt);
     std::map<const float*, ActPlanes> planes;      // 16-bit hi/lo planes of the tensors BF kernels read (key: base pointer)
     std::set<const float*> fresh;                  // planes already written by a conv epilogue in the current pass
     std::vector<BfPrepJob> bf_jobs; std::vector<int> bf_job_begin, bf_job_end;
@@ -129,9 +135,10 @@ struct Engine {
     float act_scale;                                  // power-of-two scale of the fp16 forward planes (per network)
     int ensure_planes(const TView& v, const ActPlanes* pl, cudaStream_t st);
     void planes_written(const TView& v, const ActPlanes* pl, bool written);
-    bool fwd_args(const ConvLayer& L, const TView& x, const TView& y, ConvGemm& p) const;
-    bool dgrad_args(const ConvLayer& L, const TView& dpre, const TView& dx, ConvGemm& p) const;
-    bool wgrad_args(const ConvLayer& L, const TView& x, const TView& dpre, ConvWgrad& q) const;
+    // kernel arguments of layer li's three directions on its planned views; false: the views do not fit the layer
+    bool fwd_args(int li, ConvGemm& p) const;
+    bool dgrad_args(int li, ConvGemm& p) const;
+    bool wgrad_args(int li, ConvWgrad& q) const;
     int wgrad(const ConvLayer& L, const ConvPlan& P, const ConvWgrad& q, cudaStream_t st);
     // ---- data-parallel exchange over NVLink peer memory (csrc/dp.cu)
     int dp_rank, dp_world; bool dp_connected;
@@ -200,10 +207,12 @@ struct Engine {
     void layout_dispnet(Bump& A);
     int forward_dispnet(int disp_mask, cudaStream_t st);
     int backward_dispnet(cudaStream_t st);
-    int deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, int dx_acc, cudaStream_t st);
+    int deconv_bwd(int li, int dx_acc, cudaStream_t st);
 
     Engine();
-    size_t layout(float* base);      // returns floats needed; base == nullptr: sizing only (the views are not usable)
+    // *floats: the workspace floats needed; base == nullptr: sizing only (the views are not usable).  -2: a layer's
+    // planned views do not fit it
+    int layout(float* base, size_t* floats);
     int build_madnet();
     int finalize_groups(const int* group_of_layer, int n_groups);
 
@@ -220,10 +229,9 @@ struct Engine {
     int backward(int mode, int group, cudaStream_t st);     // mode 1 = MAD(group), 2 = FULL
     int update(int group, float lr, float mu, float gscale, cudaStream_t st);
 
-    // helpers
-    int conv_fwd(const ConvLayer& L, const TView& x, const TView& y, const float* res, int res_cs, cudaStream_t st);
-    int conv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, const TView* dx_mask,
-                 float mask_alpha, int dx_acc, int want_wgrad, cudaStream_t st);
+    // helpers: layer li on the views its plan holds
+    int conv_fwd(int li, const float* res, int res_cs, cudaStream_t st);
+    int conv_bwd(int li, int want_dx, float dx_slope, int dx_acc, int want_wgrad, cudaStream_t st);
     bool trainable(int layer, int mode, int group) const;
 };
 

@@ -101,10 +101,9 @@ void Engine::layout_dispnet(Bump& A) {
 
 int Engine::forward_dispnet(int disp_mask, cudaStream_t st) {
     const int nd = 2 * DN_MAXD + 1;
-    if (conv_fwd(layers[0], img, d_c1, nullptr, 0, st)) return -1;
-    if (conv_fwd(layers[1], d_c1, d_c2, nullptr, 0, st)) return -1;
+    for (int li = 0; li < 3; ++li)          // conv1, conv2, conv_redir
+        if (conv_fwd(li, nullptr, 0, st)) return -1;
     TView c2a = batch(d_c2, 0, B), c2b = batch(d_c2, B, B);
-    if (conv_fwd(layers[2], c2a, slice(d_cat3, nd, 64), nullptr, 0, st)) return -1;
     {
         CorrFwd cf{};
         cf.left = c2a.p; cf.lcs = c2a.cs; cf.right = c2b.p; cf.rcs = c2b.cs; cf.u = nullptr; cf.ucs = 0;
@@ -117,24 +116,16 @@ int Engine::forward_dispnet(int disp_mask, cudaStream_t st) {
         prof_note(0, (double)B * cf.h * cf.w * (2.0 * 128 + nd) * 4.0);
         if (rc) return -1;
     }
-    TView x = d_cat3;
-    for (int i = 0; i < 8; ++i) {
-        if (conv_fwd(layers[3 + i], x, d_enc[i], nullptr, 0, st)) return -1;
-        x = d_enc[i];
-    }
+    for (int i = 0; i < 8; ++i)
+        if (conv_fwd(3 + i, nullptr, 0, st)) return -1;
     const TView skips[5] = {d_enc[5], d_enc[3], d_enc[1], c2a, batch(d_c1, 0, B)};
-    TView bottom = d_enc[7];
     for (int u = 0; u < 5; ++u) {
-        const UpSpec& S = DN_UP[u];
-        TView cat = d_cat[u];
-        if (add_channels(cat.p, cat.cs, skips[u].p, skips[u].cs, cat.pixels(), S.skip, 1.f, 0, st)) return -1;   // tf.concat copy
-        if (conv_fwd(layers[up_layer(u, 0)], bottom, slice(cat, S.skip, S.cout), nullptr, 0, st)) return -1;
-        if (conv_fwd(layers[up_layer(u, 1)], bottom, d_pr[u], nullptr, 0, st)) return -1;
-        if (conv_fwd(layers[up_layer(u, 2)], d_pr[u], slice(cat, S.skip + S.cout, 1), nullptr, 0, st)) return -1;
-        if (conv_fwd(layers[up_layer(u, 3)], cat, d_cc[u], nullptr, 0, st)) return -1;
-        bottom = d_cc[u];
+        const TView& cat = d_cat[u];
+        if (add_channels(cat.p, cat.cs, skips[u].p, skips[u].cs, cat.pixels(), DN_UP[u].skip, 1.f, 0, st)) return -1;   // tf.concat copy
+        for (int j = 0; j < 4; ++j)         // deconv, predict, up_predict, concat
+            if (conv_fwd(up_layer(u, j), nullptr, 0, st)) return -1;
     }
-    if (conv_fwd(layers[DN_PRED], d_cc[4], d_pred, nullptr, 0, st)) return -1;
+    if (conv_fwd(DN_PRED, nullptr, 0, st)) return -1;
     for (int i = 0; i < 7; ++i) {
         if (!(disp_mask & (1 << i))) continue;
         const TView& src = i < 5 ? d_pr[i] : d_pred;
@@ -147,37 +138,36 @@ int Engine::forward_dispnet(int disp_mask, cudaStream_t st) {
     return 0;
 }
 
-// conv2d_transpose backward.  x: its input [n,h,w,cin]; dpre: grad wrt pre-activation output [n,2h,2w,cout].
+// conv2d_transpose backward of layer li, always with its weight gradient and with the input gradient into its planned dx
+// (dx_acc: added to it).  x: its input [n,h,w,cin]; dpre: grad wrt pre-activation output [n,2h,2w,cout].
 //   dW[kh,kw,cout,cin] = wgrad of the stride-2 conv that maps the big map (channels cout) to the small one (channels cin)
 //   dx                 = that stride-2 conv applied to dpre with the same (canonical) weights as HWIO [.,.,cout,cin]
-int Engine::deconv_bwd(const ConvLayer& L, const TView& x, const TView& dpre, const TView* dx, int dx_acc, cudaStream_t st) {
-    const int li = (int)(&L - &layers[0]);
+int Engine::deconv_bwd(int li, int dx_acc, cudaStream_t st) {
+    const ConvLayer& L = layers[li];
     const ConvPlan& P = plan[li];
     MS_REQUIRE(L.transposed, "deconv_bwd: not a transposed layer");
+    MS_REQUIRE(P.dx.p, "deconv_bwd: layer " + L.name + " has no planned input gradient");
     ConvWgrad q;
     ConvGemm p;
-    MS_REQUIRE(same_view(x, P.x) && same_view(dpre, P.dpre) && wgrad_args(L, x, dpre, q) &&
-               (!dx || (same_view(*dx, P.dx) && dgrad_args(L, dpre, *dx, p))), "deconv_bwd: views differ from the layer's plan");
-    if (P.dp) { fresh.erase(dpre.p); if (ensure_planes(dpre, P.dp, st)) return -1; }     // bf16 planes of the big map's gradient
+    wgrad_args(li, q);                      // (both fit: plan_convs checked the plan's views)
+    dgrad_args(li, p);
+    if (P.dp) { fresh.erase(P.dpre.p); if (ensure_planes(P.dpre, P.dp, st)) return -1; }     // bf16 planes of the big map's gradient
     {
         prof_begin(CAT_CONV_WGRAD, st, li);
         int rc = wgrad(L, P, q, st);
-        if (!rc) rc = bias_grad(dpre, Gr + L.b_off, wg_ws, wg_ws_floats, st);
+        if (!rc) rc = bias_grad(P.dpre, Gr + L.b_off, wg_ws, wg_ws_floats, st);
         prof_end(st);
-        prof_note((double)x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
+        prof_note((double)P.x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
         if (rc) return -1;
     }
-    if (dx) {
-        p.accumulate = dx_acc;
-        prof_begin(CAT_CONV_DGRAD, st, li);
-        // (an accumulating launch would leave dx's own planes stale: it writes none)
-        const int rc = P.dgrad == ConvPlan::DGRAD_BF ? conv_bf(p, *P.dp, P.tiles[1], nullptr, sk().bf_part, sk().bf_tickets, st) : conv_gemm(p, st);
-        planes_written(*dx, P.dxp, false);
-        prof_end(st);
-        prof_note((double)x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
-        if (rc) return -1;
-    }
-    return 0;
+    p.accumulate = dx_acc;
+    prof_begin(CAT_CONV_DGRAD, st, li);
+    // (an accumulating launch would leave dx's own planes stale: it writes none)
+    const int rc = P.dgrad == ConvPlan::DGRAD_BF ? conv_bf(p, *P.dp, P.tiles[1], nullptr, sk().bf_part, sk().bf_tickets, st) : conv_gemm(p, st);
+    planes_written(P.dx, P.dxp, false);
+    prof_end(st);
+    prof_note((double)P.x.pixels() * L.kh * L.kw * L.cin * L.cout, 0);
+    return rc ? -1 : 0;
 }
 
 int Engine::backward_dispnet(cudaStream_t st) {
@@ -186,32 +176,27 @@ int Engine::backward_dispnet(cudaStream_t st) {
     if (resize_bilinear_bwd(g_disp.p, 1, d_pred.p, d_pred.cs, B, d_pred.h, d_pred.w, gd_pred.p, 1, Hp, Wp, H, W, 1.f, 0, 2.f, 0,
                             0, rs_tmp, st)) return -1;
     // prediction conv (linear): -> grad of up1/concat output
-    if (conv_bwd(layers[DN_PRED], d_cc[4], gd_pred, &gd_cc[4], nullptr, 1.f, 0, 1, st)) return -1;
+    if (conv_bwd(DN_PRED, 1, 1.f, 0, 1, st)) return -1;
 
-    TView c2a = batch(d_c2, 0, B);
     for (int u = 4; u >= 0; --u) {
         const UpSpec& S = DN_UP[u];
-        const TView bottom = u == 0 ? d_enc[7] : d_cc[u - 1];
-        TView gbottom = u == 0 ? gd_enc[7] : gd_cc[u - 1];
         // concat conv (linear): dpre = gd_cc[u] ; input = d_cat[u]
-        if (conv_bwd(layers[up_layer(u, 3)], d_cat[u], gd_cc[u], &gd_cat[u], nullptr, 1.f, 0, 1, st)) return -1;
-        TView g_dec = slice(gd_cat[u], S.skip, S.cout), g_up = slice(gd_cat[u], S.skip + S.cout, 1);
-        TView dec_act = slice(d_cat[u], S.skip, S.cout);
+        if (conv_bwd(up_layer(u, 3), 1, 1.f, 0, 1, st)) return -1;
+        TView g_dec = slice(gd_cat[u], S.skip, S.cout), dec_act = slice(d_cat[u], S.skip, S.cout);
         if (leaky_bwd(g_dec.p, g_dec.cs, dec_act.p, dec_act.cs, g_dec.pixels(), S.cout, DN_ALPHA, st)) return -1;
         // up_predict (transposed, linear): input = predict output
-        if (deconv_bwd(layers[up_layer(u, 2)], d_pr[u], g_up, &gd_pr[u], 0, st)) return -1;
-        // predict conv (linear): dpre = gd_pr[u] -> gbottom (write)
-        if (conv_bwd(layers[up_layer(u, 1)], bottom, gd_pr[u], &gbottom, nullptr, 1.f, 0, 1, st)) return -1;
-        // deconv (transposed, leaky already applied): -> gbottom (accumulate)
-        if (deconv_bwd(layers[up_layer(u, 0)], bottom, g_dec, &gbottom, 1, st)) return -1;
+        if (deconv_bwd(up_layer(u, 2), 0, st)) return -1;
+        // predict conv (linear): dpre = gd_pr[u] -> grad of the bottom (write)
+        if (conv_bwd(up_layer(u, 1), 1, 1.f, 0, 1, st)) return -1;
+        // deconv (transposed, leaky already applied): -> grad of the bottom (accumulate)
+        if (deconv_bwd(up_layer(u, 0), 1, st)) return -1;
     }
     // ---- encoder, top down.  gd_enc[7] = d(conv6/1 output) complete.
     // feature grads that also receive a skip-slice contribution: enc[5] (up5), enc[3] (up4), enc[1] (up3)
     auto skip_slice = [&](int u) { return slice(gd_cat[u], 0, DN_UP[u].skip); };
     if (leaky_bwd(gd_enc[7].p, gd_enc[7].cs, d_enc[7].p, d_enc[7].cs, gd_enc[7].pixels(), gd_enc[7].c, DN_ALPHA, st)) return -1;
     for (int i = 7; i >= 0; --i) {
-        const TView xin = i == 0 ? d_cat3 : d_enc[i - 1];
-        TView dx = i == 0 ? gd_cat3 : gd_enc[i - 1];
+        const TView& dx = i == 0 ? gd_cat3 : gd_enc[i - 1];
         int acc = 0;
         const int below = i - 1;              // index of the feature receiving dx
         int skip_u = below == 5 ? 0 : (below == 3 ? 1 : (below == 1 ? 2 : -1));
@@ -220,17 +205,16 @@ int Engine::backward_dispnet(cudaStream_t st) {
             if (add_channels(dx.p, dx.cs, sl.p, sl.cs, dx.pixels(), dx.c, 1.f, 0, st)) return -1;
             acc = 1;
         }
-        TView mask = i == 0 ? d_cat3 : d_enc[i - 1];
-        if (conv_bwd(layers[3 + i], xin, gd_enc[i], &dx, i == 0 ? nullptr : &mask, DN_ALPHA, acc, 1, st)) return -1;
+        if (conv_bwd(3 + i, 1, i == 0 ? 1.f : DN_ALPHA, acc, 1, st)) return -1;
     }
     // gd_cat3: [0,81) corr grads (linear), [81,145) conv_redir output grads (leaky)
     {
         TView g_red = slice(gd_cat3, nd, 64), red_act = slice(d_cat3, nd, 64);
         if (leaky_bwd(g_red.p, g_red.cs, red_act.p, red_act.cs, g_red.pixels(), 64, DN_ALPHA, st)) return -1;
         TView gc2a = batch(gd_c2, 0, B), gc2b = batch(gd_c2, B, B);
-        if (conv_bwd(layers[2], c2a, g_red, &gc2a, nullptr, 1.f, 0, 1, st)) return -1;           // writes d(conv2a)
+        if (conv_bwd(2, 1, 1.f, 0, 1, st)) return -1;           // conv_redir: writes d(conv2a)
         CorrBwd cb{};
-        TView c2b = batch(d_c2, B, B);
+        TView c2a = batch(d_c2, 0, B), c2b = batch(d_c2, B, B);
         cb.left = c2a.p; cb.lcs = c2a.cs; cb.right = c2b.p; cb.rcs = c2b.cs; cb.u = nullptr; cb.ucs = 0;
         cb.dcost = gd_cat3.p; cb.dcs = gd_cat3.cs; cb.dleft = gc2a.p; cb.dlcs = gc2a.cs; cb.dright = gc2b.p; cb.drcs = gc2b.cs;
         cb.du = nullptr; cb.ducs = 0;
@@ -246,13 +230,13 @@ int Engine::backward_dispnet(cudaStream_t st) {
     }
     if (leaky_bwd(gd_c2.p, gd_c2.cs, d_c2.p, d_c2.cs, gd_c2.pixels(), 128, DN_ALPHA, st)) return -1;
     // conv2 (shared, batch 2B): wgrad + dgrad -> gd_c1 ; then the up1 skip (conv1a) ; then leaky
-    if (conv_bwd(layers[1], d_c1, gd_c2, &gd_c1, nullptr, 1.f, 0, 1, st)) return -1;
+    if (conv_bwd(1, 1, 1.f, 0, 1, st)) return -1;
     {
         TView gc1a = batch(gd_c1, 0, B), sl = skip_slice(4);
         if (add_channels(gc1a.p, gc1a.cs, sl.p, sl.cs, gc1a.pixels(), 64, 1.f, 1, st)) return -1;
     }
     if (leaky_bwd(gd_c1.p, gd_c1.cs, d_c1.p, d_c1.cs, gd_c1.pixels(), 64, DN_ALPHA, st)) return -1;
-    return conv_bwd(layers[0], img, gd_c1, nullptr, nullptr, 1.f, 0, 1, st);
+    return conv_bwd(0, 0, 1.f, 0, 1, st);
 }
 
 }  // namespace ms

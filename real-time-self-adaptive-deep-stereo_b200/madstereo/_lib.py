@@ -33,14 +33,7 @@ _SIGS = {
     'ms_conv2d_bf_scratch': (Z, [I, I, I, I, I, I, I]),
     'ms_conv2d_wgrad_bf': (I, [P, I, I, I, I, I, P, I, I, I, I, P, P, I, I, I, I, P, Z, P]),
     'ms_conv2d_wgrad_bf_scratch': (Z, [I, I, I, I, I, I, I, I, I]),
-    'ms_bf_split': (I, [P, I, I, I, I, I, P, P, I, I, F, P]),
     'ms_bf_weight_halfs': (Z, [I, I, I]),
-    'ms_bf_prep_weights': (I, [P, I, I, I, I, I, P, P, P]),
-    'ms_conv2d_fwd_bf_planes': (I, [P, P, I, I, F, I, I, I, I, P, P, P, I, I, P, P, I, I, I, I, I, F, P, P, P]),
-    'ms_conv2d_bf_part_floats': (Z, []),
-    'ms_conv2d_bf_ticket_words': (Z, []),
-    'ms_conv2d_wgrad_bf_planes': (I, [P, P, I, I, I, I, I, P, P, I, I, I, I, P, P, I, I, I, I, P, Z, P]),
-    'ms_conv2d_wgrad_bf_workspace': (Z, [I, I, I, I]),
     'ms_conv2d_wgrad_workspace': (Z, [I, I, I, I, Z]),
     'ms_conv2d_wgrad': (I, [P, I, I, I, I, I, P, I, I, I, I, P, P, I, I, I, I, P, Z, P]),
     'ms_conv2d_transpose_fwd': (I, [P, I, I, I, I, I, P, P, P, I, I, I, I, I, F, P, P]),

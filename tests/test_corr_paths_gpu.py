@@ -246,15 +246,30 @@ def test_corr_bwd(lib, name):
 
 
 # --------------------------------------------------------------------------------------------------------- dispatch
-def _cuda_kernels(fn):
-    """Names of the CUDA kernels fn launches (torch.profiler, CUDA activity); None if the profiler records none."""
+def _cuda_kernels(fn, sessions=4):
+    """Names of the CUDA kernels one call of fn launches (torch.profiler, CUDA activity); None if the profiler records none.
+
+    A session can miss its first activities when the profiler has run before in the same process -- for a call that
+    launches one kernel, all of it -- so fn runs twice with a torch kernel in between as a marker, and only what follows
+    the marker counts (as in cuda_activities of tests/golden/make_engine_kernels.py; fn only rewrites its outputs).  Now
+    and then a session records no CUDA activity at all; it is repeated before concluding that the profiler sees none."""
     from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
+    for _ in range(sessions):
         torch.cuda.synchronize()
-    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return names or None
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+            torch.ones(1, device='cuda').add_(1)
+            torch.cuda.synchronize()
+            fn()
+            torch.cuda.synchronize()
+        ev = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA),
+                    key=lambda e: e.time_range.start)
+        names = [e.name for e in ev]
+        marks = [i for i, n in enumerate(names) if 'ms::' not in n]
+        if marks:
+            return names[marks[-1] + 1:]
+    return None
 
 
 CORR_KERNELS = ('corr_fwd_kernel(', 'corr_fwd2_kernel<', 'corr_fwd3_kernel<', 'corr_fwd4_kernel<', 'corr_mma_kernel',

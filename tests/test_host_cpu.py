@@ -1,6 +1,7 @@
 """CPU tests of the host side: C-ABI exports, layer/group tables through the engine (no kernels run),
 samplers and the reward recurrence against the oracle transcription."""
 import ctypes
+import importlib.util
 import json
 import os
 import re
@@ -13,6 +14,10 @@ from madstereo import _lib
 from oracle import adaptation as OA
 from oracle.madnet import param_shapes, mad_groups_full
 from Sampler import sampler_factory
+
+_spec = importlib.util.spec_from_file_location('make_engine_kernels', os.path.join(ROOT, 'tests', 'golden', 'make_engine_kernels.py'))
+_mk = importlib.util.module_from_spec(_spec)
+_spec.loader.exec_module(_mk)
 
 
 def test_library_exports_every_declared_symbol():
@@ -69,10 +74,11 @@ def test_ctypes_table_matches_the_header_prototypes():
     assert seen == set(_lib._SIGS), sorted(set(_lib._SIGS) - seen)
 
 
-def _engine_tables(groups_cfg):
+def _engine_tables(groups_cfg, net='MADNet', batch=1, h=384, w=1280, variant=(2, 1, True)):
     L = _lib.lib()
-    e = L.ms_engine_create(b'MADNet', 1, 384, 1280, 2, 1, 1)
-    assert e
+    radius_d, stride, warping = variant
+    e = L.ms_engine_create(net.encode(), batch, h, w, radius_d, stride, int(warping))
+    assert e, L.ms_last_error()
     n = L.ms_engine_num_layers(e)
     layers = []
     for i in range(n):
@@ -88,7 +94,7 @@ def _engine_tables(groups_cfg):
                 arr[name_to_idx[nm]] = g
     assert L.ms_engine_set_groups(e, arr, n, len(groups_cfg)) == 0
     npar, nws = ctypes.c_size_t(), ctypes.c_size_t()
-    assert L.ms_engine_sizes(e, ctypes.byref(npar), ctypes.byref(nws)) == 0
+    assert L.ms_engine_sizes(e, ctypes.byref(npar), ctypes.byref(nws)) == 0, L.ms_last_error()
     ranges = []
     for g in range(len(groups_cfg)):
         b, en = ctypes.c_size_t(), ctypes.c_size_t()
@@ -124,6 +130,17 @@ def test_engine_layer_table_matches_reference_variable_names():
         assert e0 == b1
     # 16-byte alignment of every tensor (float4 loads)
     assert all(w % 4 == 0 and b % 4 == 0 for w, b in offs)
+
+
+@pytest.mark.parametrize('cfg', _mk.CONFIGS, ids=[c[0] for c in _mk.CONFIGS])
+def test_engine_sizes_every_kernel_sequence_config(cfg):
+    """ms_engine_sizes lays the engine out without a device, and the layout checks every layer's planned views against
+    the layer: MADNet with its MAD modules at the radius / stride / warping variants, and DispNet."""
+    _name, net, batch, h, w, variant, _steps = cfg
+    groups = json.load(open(os.path.join(PKG, 'block_config', 'MadNet_full.json'))) if net == 'MADNet' else []
+    layers, npar, nws, _ranges, _offs = _engine_tables(groups, net, batch, h, w, variant or (2, 1, True))
+    assert len(layers) == (49 if net == 'MADNet' else 32)
+    assert npar > 0 and nws > 0
 
 
 def test_unknown_network_name():
