@@ -174,6 +174,26 @@ int ms_rectify_u8(const unsigned char* src, const float* map, int B, int h, int 
 int ms_pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int Hp, int Wp, int dst_cs,
                    float scale, float bias, void* stream);
 
+/* Replaces preprocessing.colorize_img (Data_utils/preprocessing.py:91-117) as the summaries of Stereo_Online_Adaptation.py
+ * (:131-140) and Stereo_Continual_Adaptation.py (:135-145) call it: value [B,H,W,1] (DEVICE) -> out [B,H,W,3] float, the
+ * lut [256,3] (DEVICE, float32: matplotlib's colormap at np.arange(256), RGB) gathered at
+ *   k = to_int32(round(((value - vmin) / (vmax - vmin)) * 255)),  round = half to even,
+ * each operation rounded in float32 as the reference graph computes it.  vmin / vmax default (use_* == 0) to the min / max
+ * over the whole batch; with both given no reduction runs.  An index outside [0, 255] gives 0 in every channel, as TF's GPU
+ * gather does; a constant map (vmax == vmin: 0/0) has no index and comes out black.  workspace: device floats, at least
+ * ms_colorize_workspace_floats(). */
+size_t ms_colorize_workspace_floats(void);
+int ms_colorize(const float* value, int B, int H, int W, const float* lut, int use_vmin, float vmin, int use_vmax, float vmax,
+                float* out, float* workspace, size_t workspace_floats, void* stream);
+/* Replaces tf.summary.image(name, preprocessing.colorize_img(value, cmap=...), max_outputs=1) up to the PNG encoding
+ * (Stereo_Online_Adaptation.py:135-136, Stereo_Continual_Adaptation.py:139-141): vmin / vmax over the whole batch as
+ * ms_colorize, then image 0 only, normalized to uint8 out [H,W,3] (DEVICE, RGB) as TF's ImageSummary normalizes float images:
+ * over the finite pixels, min >= 0 scales by 255 / max (0 if max < 1e-6), otherwise by 127 / max(|min|, |max|) plus 128;
+ * c * scale and + offset each rounded in float32, then truncated toward zero; a non-finite pixel is red (bad_color).  That
+ * rounding is restated from TF's documented behaviour, not checked against its kernel. */
+int ms_colorize_summary_u8(const float* value, int B, int H, int W, const float* lut, int use_vmin, float vmin, int use_vmax,
+                           float vmax, unsigned char* out, float* workspace, size_t workspace_floats, void* stream);
+
 /* ---- engine level: what one sess.run(fetches) does (Stereo_Online_Adaptation.py:194-208) ---------- */
 
 /* Replaces Nets.get_stereo_net(name,args) graph construction (Nets/__init__.py:9-13, Nets/MadNet.py:251-364).

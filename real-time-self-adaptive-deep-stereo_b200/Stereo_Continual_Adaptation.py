@@ -7,7 +7,9 @@ op only every `--dilation` frames (:212), the reward recurrence with --decay / -
 (:269-271) and the output files (`overall.csv`, `series.csv`, `histogram.csv`, `disparities/disparity_<step>.png`,
 `weights/`).  Underneath: Nets.get_stereo_net + madstereo.adaptation.OnlineAdaptation(loss='proxy', ...).step, the masked-L1
 loss is csrc/loss.cu:proxy_loss.  --reprojectionScale s compares the MAD module disparities with the proxy resized to 1/s
-and divided by s (:95-112); --summary is accepted but not written (as in the online driver).
+and divided by s (:95-112).  --summary writes the reference's TensorBoard summaries every 100 frames (:135-145, :207-209,
+:259-260): scalars `EPE` and `bad3` (the engine's masked mean |d - gt| and fraction > 3 px, computed on those frames only),
+images `full_res_disp/image`, `proxy_disp/image` and `gt_disp/image`, as the online driver writes them.
 
     python Stereo_Continual_Adaptation.py -l list.csv -o out --weights ckpt --modelName MADNet \
         --blockConfig block_config/MadNet_full.json --mode MAD --sampleMode PROBABILITY --dilation 1
@@ -27,6 +29,7 @@ if HERE not in sys.path:
 import Nets  # noqa: E402
 from Data_utils import data_reader, weights_utils  # noqa: E402
 import Stereo_Online_Adaptation as online  # noqa: E402
+from madstereo.summary import AdaptationSummary  # noqa: E402
 
 MAX_DISP = 256
 PIXEL_TH = 3
@@ -75,13 +78,19 @@ def build_model(args, train_config):
     return stereo_net, adapt
 
 
-def run_loop(adapt, frames, args, get_disparity, log=print):
-    """The reference's while-loop (:183-282) around `adapt.step`; `frames` yields (left, right, gt, proxy, real_width)."""
+def run_loop(adapt, frames, args, get_disparity, log=print, summary=None, disparity_map=None):
+    """The reference's while-loop (:183-282) around `adapt.step`; `frames` yields (left, right, gt, proxy, real_width).
+    `summary` (an AdaptationSummary, or None): at every 100th step the engine also computes EPE / bad3 against gt, and
+    they go to the summary with `disparity_map()`, the proxy and the ground truth."""
     avg_accumulator, d1_accumulator = [], []
     step = 0
     start_time = time.time()
     for left, right, gt, proxy, _real_width in frames:
-        adapt.step(left, right, None, want_disp_mask=0b100000, proxy=proxy)
+        summary_now = summary is not None and summary.due(step)
+        out = adapt.step(left, right, gt if summary_now else None, want_disp_mask=0b100000, proxy=proxy)
+        if summary_now:
+            summary.add(step, out['epe'], out['bad3'], [('full_res_disp', disparity_map()), ('proxy_disp', proxy),
+                                                        ('gt_disp', gt)])
         disp = get_disparity()[-1]
         epe, d1 = frame_errors(disp, np.asarray(gt)[-1])
         d1_accumulator.append(d1)
@@ -109,7 +118,8 @@ def write_outputs(args, avg_accumulator, d1_accumulator):
             f_out.write('%d & %.3f & %.3f\n' % (i, a, b))
 
 
-def main(args, build=build_model):
+def main(args, build=build_model, colorize=None):
+    """`build` and `colorize` (the summary images' colour map, default the GPU kernel) can be replaced by tests."""
     with open(args.blockConfig) as json_data:
         train_config = json.load(json_data)
     online.check_reprojection_scale(args)
@@ -126,7 +136,13 @@ def main(args, build=build_model):
     assert (len(w_dict) > 0)
     adapt.load_weights(w_dict, strict=False)
     print('Disparity Net Restored?: {}, number of restored variables: {}'.format(True, len(w_dict)))
-    avg, d1, step, _ = run_loop(adapt, data_set, args, get_disparity=lambda: predictions[-1].numpy())
+    summary = AdaptationSummary(args.output, colorize) if args.summary else None
+    try:
+        avg, d1, step, _ = run_loop(adapt, data_set, args, get_disparity=lambda: predictions[-1].numpy(), summary=summary,
+                                    disparity_map=lambda: predictions[-1].tensor())
+    finally:
+        if summary is not None:
+            summary.close()
     print(adapt.fetch_counter)
     write_outputs(args, avg, d1)
     if args.saveWeights:
@@ -140,8 +156,6 @@ def main(args, build=build_model):
 if __name__ == '__main__':
     parser = build_parser()
     args = parser.parse_args()
-    if args.summary:
-        print('WARNING: --summary is accepted for command-line compatibility, but no TensorBoard summaries are written')
     if not os.path.exists(args.output):
         os.makedirs(args.output)
     if args.logDispStep != -1 and not os.path.exists(os.path.join(args.output, 'disparities')):

@@ -5,9 +5,12 @@ Mirrors Stereo_Online_Adaptation.py of the reference: the same flags (:290-307),
 same loop (:176-253).  What changed underneath: the graph construction and `sess.run` are `Nets.get_stereo_net` +
 `madstereo.adaptation.OnlineAdaptation.step` (sampling, reward recurrence, reset and the CUDA step live there), the
 `tf.data` reader is Data_utils/data_reader.py (host thread + pinned buffers; the next frame's copy overlaps the current
-frame), `--weights` accepts a TensorFlow V2 checkpoint prefix or directory (read without TensorFlow) or an `.npz`, and
-TensorBoard summaries (`--summary`) are accepted but not written.  `--reprojectionScale s` computes the MAD module losses at
-1/s resolution as the reference does (:22-23, :91-107), disparity units included; it has no effect under FULL / NONE.
+frame), and `--weights` accepts a TensorFlow V2 checkpoint prefix or directory (read without TensorFlow) or an `.npz`.
+`--reprojectionScale s` computes the MAD module losses at 1/s resolution as the reference does (:22-23, :91-107), disparity
+units included; it has no effect under FULL / NONE.  `--summary` writes the reference's TensorBoard summaries (:131-140,
+:196-199, :235-236) to an events file in the output folder every 100 frames: scalars `EPE` and `bad3`, and images
+`full_res_disp/image` and `gt_disp/image` (the jet-colorized pre-update disparity and ground truth of frame 0 of the batch,
+colorized on the GPU by madstereo.ops.colorize_summary_image), written by madstereo.summary without TensorFlow.
 
     python Stereo_Online_Adaptation.py -l list.csv -o out --weights ckpt/MADNet/kitti/weights.ckpt \\
         --modelName MADNet --blockConfig block_config/MadNet_full.json --mode MAD --sampleMode PROBABILITY
@@ -29,6 +32,7 @@ if HERE not in sys.path:
 import Nets  # noqa: E402
 from Data_utils import data_reader, weights_utils  # noqa: E402
 from Sampler import sampler_factory  # noqa: E402
+from madstereo.summary import AdaptationSummary  # noqa: E402
 
 # static params
 MAX_DISP = 256
@@ -98,9 +102,10 @@ def save_disparity(path, dispy):
     cv2.imwrite(path, dispy_to_save)
 
 
-def run_loop(adapt, frames, args, max_steps, get_disparity=None, log=print):
+def run_loop(adapt, frames, args, max_steps, get_disparity=None, log=print, summary=None, disparity_map=None):
     """The reference's while-loop (:176-253) around `adapt.step` (== one sess.run).  `frames` yields (left, right, gt)
-    batches; returns the accumulators the writers need."""
+    batches; returns the accumulators the writers need.  `summary` (an AdaptationSummary, or None) gets this step's EPE /
+    bad3, the full-resolution disparity `disparity_map()` and the ground truth at every 100th step."""
     epe_accumulator, bad3_accumulator = [], []
     exec_time = 0
     step = 0
@@ -122,6 +127,8 @@ def run_loop(adapt, frames, args, max_steps, get_disparity=None, log=print):
             log('Step:{:4d}\tbad3:{:.2f}\tEPE:{:.2f}\tSSIM:{:.2f}\tf/b time:{:3f}\tMissing time:{}'.format(
                 step, out['bad3'], out['epe'], out['loss'], fbTime, datetime.timedelta(seconds=missing_time)))
             start_time = time.time()
+        if summary is not None and summary.due(step):
+            summary.add(step, out['epe'], out['bad3'], [('full_res_disp', disparity_map()), ('gt_disp', gt)])
         if args.logDispStep != -1 and step % args.logDispStep == 0 and get_disparity is not None:
             save_disparity(os.path.join(args.output, 'disparities/disparity_{}.png'.format(step)), get_disparity()[0])
         step += 1
@@ -160,7 +167,8 @@ def check_reprojection_scale(args):
                          % (args.reprojectionScale, args.modelName))
 
 
-def main(args, build=build_model):
+def main(args, build=build_model, colorize=None):
+    """`build` and `colorize` (the summary images' colour map, default the GPU kernel) can be replaced by tests."""
     with open(args.blockConfig) as json_data:
         train_config = json.load(json_data)
     check_reprojection_scale(args)
@@ -182,8 +190,14 @@ def main(args, build=build_model):
     print('Disparity Net Restored?: {}, number of restored variables: {}'.format(True, len(w_dict)))
 
     max_steps = data_set.get_max_steps()
-    epe_array, bad3_array, exec_time, step = run_loop(adapt, data_set, args, max_steps,
-                                                      get_disparity=lambda: predictions[-1].numpy())
+    summary = AdaptationSummary(args.output, colorize) if args.summary else None
+    try:
+        epe_array, bad3_array, exec_time, step = run_loop(adapt, data_set, args, max_steps,
+                                                          get_disparity=lambda: predictions[-1].numpy(), summary=summary,
+                                                          disparity_map=lambda: predictions[-1].tensor())
+    finally:
+        if summary is not None:
+            summary.close()
     write_stats(os.path.join(args.output, 'stats.csv'), epe_array, bad3_array, exec_time, step, adapt.reset_counter,
                 len(predictions[:-1]) if args.mode == 'MAD' else len(predictions), adapt.fetch_counter, adapt.sample_distribution)
     write_series(os.path.join(args.output, 'series.csv'), epe_array, bad3_array, exec_time, step)
@@ -194,8 +208,6 @@ def main(args, build=build_model):
 if __name__ == '__main__':
     parser = build_parser()
     args = parser.parse_args()
-    if args.summary:
-        print('WARNING: --summary is accepted for command-line compatibility, but no TensorBoard summaries are written')
     if not os.path.exists(args.output):
         os.makedirs(args.output)
     if args.logDispStep != -1 and not os.path.exists(os.path.join(args.output, 'disparities')):

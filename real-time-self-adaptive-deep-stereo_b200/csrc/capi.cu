@@ -274,6 +274,18 @@ int ms_pad_reflect(const float* src, int B, int H, int W, int C, float* dst, int
     return pad_reflect(src, B, H, W, C, dst, Hp, Wp, dst_cs, scale, bias, S(stream));
 }
 
+size_t ms_colorize_workspace_floats(void) { return colorize_workspace_floats(); }
+
+int ms_colorize(const float* value, int B, int H, int W, const float* lut, int use_vmin, float vmin, int use_vmax, float vmax,
+                float* out, float* workspace, size_t workspace_floats, void* stream) {
+    return colorize(value, B, H, W, lut, use_vmin, vmin, use_vmax, vmax, out, workspace, workspace_floats, S(stream));
+}
+
+int ms_colorize_summary_u8(const float* value, int B, int H, int W, const float* lut, int use_vmin, float vmin, int use_vmax,
+                           float vmax, unsigned char* out, float* workspace, size_t workspace_floats, void* stream) {
+    return colorize_summary_u8(value, B, H, W, lut, use_vmin, vmin, use_vmax, vmax, out, workspace, workspace_floats, S(stream));
+}
+
 // ---- engine --------------------------------------------------------------------------------------
 void* ms_engine_create(const char* net_name, int B, int H, int W, int radius_d, int corr_stride, int warping) {
     if (!net_name || B < 1 || H < 8 || W < 8 || radius_d < 0 || corr_stride < 1) {

@@ -205,6 +205,14 @@ int u8_resize_crop(const unsigned char* left, const unsigned char* right, int B,
 int rectify_u8(const unsigned char* left, const unsigned char* right, const float* map_left, const float* map_right, int B,
                int h, int w, unsigned char* dst_left, unsigned char* dst_right, cudaStream_t st);
 
+// colour maps for the summaries (summary.cu): preprocessing.colorize_img into float [B,H,W,3], or image 0 straight to the
+// uint8 [H,W,3] pixels of tf.summary.image; lut [256,3], workspace >= colorize_workspace_floats()
+size_t colorize_workspace_floats();
+int colorize(const float* value, int B, int H, int W, const float* lut, int use_vmin, float vmin, int use_vmax, float vmax,
+             float* out, float* ws, size_t ws_floats, cudaStream_t st);
+int colorize_summary_u8(const float* value, int B, int H, int W, const float* lut, int use_vmin, float vmin, int use_vmax,
+                        float vmax, unsigned char* out, float* ws, size_t ws_floats, cudaStream_t st);
+
 // loss (loss.cu)
 struct ReprojLoss {
     const float* left; const float* right;   // [B,H,W,3], 0..255

@@ -53,6 +53,9 @@ _SIGS = {
     'ms_adam_update': (I, [P, P, P, P, P, Z, F, F, F, F, F, P]),
     'ms_rectify_u8': (I, [P, P, I, I, I, P, P]),
     'ms_pad_reflect': (I, [P, I, I, I, I, P, I, I, I, F, F, P]),
+    'ms_colorize_workspace_floats': (Z, []),
+    'ms_colorize': (I, [P, I, I, I, P, I, F, I, F, P, P, Z, P]),
+    'ms_colorize_summary_u8': (I, [P, I, I, I, P, I, F, I, F, P, P, Z, P]),
     'ms_engine_create': (P, [c_char_p, I, I, I, I, I, I]),
     'ms_engine_destroy': (I, [P]),
     'ms_engine_num_layers': (I, [P]),

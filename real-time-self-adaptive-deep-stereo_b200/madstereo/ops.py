@@ -290,3 +290,75 @@ def pad_reflect(x, factor=64, scale=1.0, bias=0.0):
     y = torch.empty(b, hp, wp, c, device=x.device, dtype=torch.float32)
     check(lib().ms_pad_reflect(_p(x), b, h, w, c, _p(y), hp, wp, c, scale, bias, _s()), 'ms_pad_reflect')
     return y
+
+
+# ---- colour maps of the summaries (csrc/summary.cu) ------------------------------------------------------------------
+# matplotlib's segment data of the two colour maps the reference can ask for: 'jet' (the drivers' summaries) and 'gray'
+# (colorize_img's default).  Per channel, rows (x, y_left, y_right) with x rising from 0 to 1.
+_SEGMENTS = {
+    'jet': ([(0.00, 0.0, 0.0), (0.35, 0.0, 0.0), (0.66, 1.0, 1.0), (0.89, 1.0, 1.0), (1.00, 0.5, 0.5)],
+            [(0.000, 0.0, 0.0), (0.125, 0.0, 0.0), (0.375, 1.0, 1.0), (0.640, 1.0, 1.0), (0.910, 0.0, 0.0), (1.000, 0.0, 0.0)],
+            [(0.00, 0.5, 0.5), (0.11, 1.0, 1.0), (0.34, 1.0, 1.0), (0.65, 0.0, 0.0), (1.00, 0.0, 0.0)]),
+    'gray': ([(0.0, 0.0, 0.0), (1.0, 1.0, 1.0)],) * 3,
+}
+_LUTS = {}
+
+
+def _sample_segments(rows, n=256):
+    """One channel of LinearSegmentedColormap(name, segments, N=n) sampled at its n entries (gamma 1): entry i sits at
+    x = i / (n - 1) and interpolates linearly between the rows around it, from the right value of the lower row to the left
+    value of the upper one; the first entry is the first row's right value, the last the last row's left value."""
+    import numpy as np
+    a = np.asarray(rows, dtype=np.float64)
+    x, y0, y1 = a[:, 0] * (n - 1), a[:, 1], a[:, 2]
+    xi = (n - 1) * np.linspace(0, 1, n)
+    j = np.searchsorted(x, xi)[1:-1]
+    t = (xi[1:-1] - x[j - 1]) / (x[j] - x[j - 1])
+    return np.clip(np.concatenate([[y1[0]], t * (y0[j] - y1[j - 1]) + y1[j - 1], [y0[-1]]]), 0.0, 1.0)
+
+
+def colormap_lut(cmap=None):
+    """[256,3] float32 RGB: `cm.get_cmap(cmap)(np.arange(256))[:, :3]` as preprocessing.colorize_img builds it
+    (Data_utils/preprocessing.py:113-115), for cmap 'jet' or 'gray' (None = 'gray')."""
+    import numpy as np
+    name = 'gray' if cmap is None else cmap
+    if name not in _SEGMENTS:
+        raise MadStereoError('colorize_img: colour map %r is not available (only %s)' % (cmap, ', '.join(sorted(_SEGMENTS))))
+    if name not in _LUTS:
+        _LUTS[name] = np.stack([_sample_segments(ch) for ch in _SEGMENTS[name]], axis=1).astype(np.float32)
+    return _LUTS[name]
+
+
+def _colorize_args(value, vmin, vmax, cmap):
+    _chk(value, 'value')
+    if value.dim() != 4 or value.shape[3] != 1:
+        raise MadStereoError('colorize_img: value must be [batch, height, width, 1], got %s' % (tuple(value.shape),))
+    lut = torch.from_numpy(colormap_lut(cmap)).to(value.device)
+    ws = torch.empty(lib().ms_colorize_workspace_floats(), device=value.device, dtype=torch.float32)
+    b, h, w, _ = value.shape
+    return (_p(value), b, h, w, _p(lut), int(vmin is not None), float(vmin or 0.0), int(vmax is not None),
+            float(vmax or 0.0)), (lut, ws)
+
+
+def colorize_img(value, vmin=None, vmax=None, cmap=None):
+    """preprocessing.colorize_img (Data_utils/preprocessing.py:91-117): value [B,H,W,1] -> float32 [B,H,W,3] colours.
+    vmin / vmax default to the min / max of the whole batch; cmap 'jet' or 'gray' (default).  Where the reference's index
+    falls outside the colour map, and everywhere in a constant map (0/0), the colour is 0: what TF's GPU gather returns."""
+    args, keep = _colorize_args(value, vmin, vmax, cmap)
+    b, h, w = value.shape[:3]
+    out = torch.empty(b, h, w, 3, device=value.device, dtype=torch.float32)
+    ws = keep[1]
+    check(lib().ms_colorize(*args, _p(out), _p(ws), ws.numel(), _s()), 'ms_colorize')
+    return out
+
+
+def colorize_summary_image(value, vmin=None, vmax=None, cmap=None):
+    """The pixels tf.summary.image(name, colorize_img(value, vmin, vmax, cmap), max_outputs=1) encodes: image 0 of the
+    colorized batch (vmin / vmax still over the whole batch), normalized to uint8 [H,W,3] RGB as TF's ImageSummary
+    normalizes float images (include/madstereo.h: ms_colorize_summary_u8)."""
+    args, keep = _colorize_args(value, vmin, vmax, cmap)
+    h, w = value.shape[1:3]
+    out = torch.empty(h, w, 3, device=value.device, dtype=torch.uint8)
+    ws = keep[1]
+    check(lib().ms_colorize_summary_u8(*args, _p(out), _p(ws), ws.numel(), _s()), 'ms_colorize_summary_u8')
+    return out
